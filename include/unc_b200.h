@@ -300,6 +300,22 @@ int unc_dtw_batch(const float *model_means_stdvs, int cost_kind, const unc_dtw_p
 void unc_dtw_release(void);
 float unc_dtw_last_kernel_ms(void);
 
+/* ---- iterative high-frequency k-mer masking of a reference (`mask-internal`) -----------------------------------
+ *   unc_mask_internal   masking/mask_internal.sh <reference> <k> <iters> <out_prefix>: per iteration `jellyfish count`
+ *                       (forward strand, no -C), the k-mer of the maximum count, masking/mask_kmers.py -k <kmer>
+ * Each iteration counts the k-mers of the whole FASTA (bases case-insensitive; any other byte, a masked position or
+ * a record boundary breaks a k-mer), takes the k-mer with the highest count -- ties go to the smallest 2-bit code
+ * (A<C<G<T, the lexicographically smallest; jellyfish's choice is its hash order) -- and replaces every position of
+ * every occurrence, overlapping ones included, by 'N'.  Iteration i's k-mer code (first base in the top bits) and
+ * count go to kmer_codes[i] / counts[i]; when no k-mer is left the loop stops and *n_done < iters.  Only the final
+ * FASTA is written to out_fasta: each header stripped, then the record's sequence on one line, '\n' line ends, every
+ * byte not masked as in the input.  UNC_E_ARG (nothing written) for k outside 1..13, iters < 1, an empty file, a
+ * first line not starting with '>' or a record without sequence; UNC_E_TOO_LARGE for 2^32 or more bases.
+ * unc_mask_last_kernel_ms: CUDA-event time of the last call's device loop. */
+int unc_mask_internal(const char *fasta_in, const char *out_fasta, uint32_t k, uint32_t iters, uint64_t *kmer_codes,
+                      uint64_t *counts, uint32_t *n_done);
+float unc_mask_last_kernel_ms(void);
+
 /* ---- fast5 input (host; no libhdf5 needed) -------------------------------------------------------------
  *   unc_fast5_open      Fast5Reader::open_next: format detection and the list of reads
  *                                                      src/fast5_reader.cpp:134-177

@@ -52,7 +52,15 @@ def get_parser(conf):
     p.add_argument("--ordered", action="store_const", const=1, default=conf.ordered, help=type(conf).ordered.__doc__)
     p.add_argument("--exact-ties", action="store_const", const=1, default=conf.exact_ties, help=type(conf).exact_ties.__doc__)
 
-    p = sp.add_parser("pafstats", help="Computes speed and accuracy of UNCALLED mappings.", formatter_class=fmt)
+    p = sp.add_parser("mask-internal", help="Iteratively masks the most frequent k-mer of a FASTA reference with N "
+                      "(masking/mask_internal.sh)", formatter_class=fmt)
+    p.add_argument("reference", type=str, help="fasta file of the reference to mask")
+    p.add_argument("k", type=int, help="k-mer length (1 to 13)")
+    p.add_argument("iters", type=int, help="number of masking iterations to run")
+    p.add_argument("out_prefix", type=str, help="output prefix: writes <out_prefix>mask<iters>.fa")
+    p.add_argument("--device", type=int, default=0, help="CUDA device")
+
+    p = sp.add_parser("pafstats",help="Computes speed and accuracy of UNCALLED mappings.", formatter_class=fmt)
     p.add_argument("infile", type=str, help="PAF file output by UNCALLED")          # uncalled/pafstats.py:165-169
     p.add_argument("-n", "--max-reads", required=False, type=int, default=None, help="Will only look at first n reads if specified")
     p.add_argument("-r", "--ref-paf", required=False, type=str, default=None, help="Reference PAF file. Will output percent true/false "
@@ -157,6 +165,14 @@ def main(argv=None):
         index_cmd(args)
     elif args.subcmd == "map":
         map_cmd(conf, args)
+    elif args.subcmd == "mask-internal":
+        from . import _native as N
+        from .mask import mask_internal
+        assert_exists(args.reference)
+        N.check(N.lib().unc_init(args.device))
+        done = mask_internal(args.reference, args.k, args.iters, args.out_prefix)
+        if len(done) < args.iters:
+            sys.stderr.write("No k-mer left to mask after %d iterations\n" % len(done))
     elif args.subcmd == "pafstats":
         from . import pafstats
         pafstats.run(args.infile, args.ref_paf, args.max_reads)

@@ -892,3 +892,4 @@ int unc_pool_last_timing(const unc_pool *P, unc_timing *t) {
 #include "unc_stream_host.inl"
 #include "unc_selfalign_host.inl"
 #include "unc_dtw_host.inl"
+#include "unc_mask_host.inl"
