@@ -939,7 +939,9 @@ struct K2Shared {          // per CTA
     u32 wk_overflow;
     u32 wl_cnt;            // deferred window look-ups of the event in flight
     u32 cnt_blocks, cnt_steps;
-    u32 tot_children[2], tot_sources[2];   // u64 as two words, written by a worker at the end
+    u32 tot_children[2], tot_sources[2];   // u64 as two words, written by a worker (k2v2: kept by worker thread 0 per event)
+    DevWork work;          // the read's workspace slot: its ten pointers are read where they are used instead of being
+                           // held in registers across the event loop (at 72 registers they would spill)
 #ifdef K2_TRK_INLINE
     u32 trk_state[24];     // the seed tracker's scalars between its per-event calls (see unc_k2_track_event)
 #endif
@@ -2317,6 +2319,7 @@ UNC_DEV DevWork unc_work_slot(const DevWork &W0, const DevWorkStrides &S, size_t
 // EXACT: the exact-ties kernel (the reference's unstable child sort reproduced, unc_pdqsort.cuh)
 template <bool EXACT = false, bool FLAGS = false>
 UNC_DEV void unc_k2_cta_main(const DevIndex &ix, const DevParams &p, const DevBatch &B, const DevWork &W, K2Shared *sh) {
+    if (c_tid() == 0) sh->work = W;                   // published by the setup's barrier
     unc_k2_cta_setup(ix, p, sh);
     u32 epoch = 0;
     for (;;) {
@@ -2325,7 +2328,7 @@ UNC_DEV void unc_k2_cta_main(const DevIndex &ix, const DevParams &p, const DevBa
         u32 r = sh->bc[0];
         c_sync();
         if (r >= B.n_reads) break;
-        unc_k2_map_read<false, EXACT, FLAGS>(ix, p, B, W, sh, r, &epoch);
+        unc_k2_map_read<false, EXACT, FLAGS>(ix, p, B, sh->work, sh, r, &epoch);
     }
 }
 
@@ -2341,7 +2344,7 @@ UNC_DEV void unc_k2_cta_main_stream(const DevIndex &ix, const DevParams &p, cons
         u32 r = sh->bc[0];
         c_sync();
         if (r >= B.n_reads) break;
-        const DevWork W = unc_work_slot(W0, S, B.chan[r]);
-        unc_k2_map_read<true, EXACT, true>(ix, p, B, W, sh, r, &epoch);
+        if (c_tid() == 0) sh->work = unc_work_slot(W0, S, B.chan[r]);   // published by unc_k2_map_read's first barrier
+        unc_k2_map_read<true, EXACT, true>(ix, p, B, sh->work, sh, r, &epoch);
     }
 }

@@ -235,6 +235,19 @@ UNC_DEV u32 k2v2_segmask(u32 start, u32 n) { return (n >= 32u ? 0xFFFFFFFFu : ((
 // consecutive ranks (the prefix sums) and a warp that reads one rank per lane... both touch distinct banks or one
 UNC_DEV u32 k2v2_slot(u32 rank) { return ((rank & 31u) << 5) | (rank >> 5); }
 
+// worker warp ww's child staging area (K2V2_STAGE_BYTES of dynamic shared memory).  Formed as sh + offset, so that
+// the compiler sees a shared-memory address (32 bits) rather than the generic pointer stored in sh->v2_stage.
+UNC_DEV uint2 *k2v2_stage(K2Shared *sh, u32 ww) {
+    const u32 off = (u32) (sh->v2_stage - (unsigned char *) sh) + ww * K2V2_STAGE_BYTES;
+    return (uint2 *) ((unsigned char *) sh + off);
+}
+
+// u64 counter kept as two u32 words in shared memory (one thread)
+UNC_DEV void k2v2_add64(u32 *w, u32 v) {
+    const u64 s = (((u64) w[1] << 32) | w[0]) + v;
+    w[0] = (u32) s; w[1] = (u32) (s >> 32);
+}
+
 // the next group of 32 bucket ranks for this warp (two sweeps of 32 groups: see phase C2)
 UNC_DEV u32 k2v2_grab(u32 *counter) {
     u32 g = 0;
@@ -370,27 +383,24 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
     const u32 maxp = p.max_paths;
     const u32 S0 = ((maxp + 31u) >> 5) * K2_CH_SLOTS;                     // record index of the first source
     const size_t gen_recs = (size_t) S0 + maxp;
-    const float scale = B.scale[r], shift = B.shift[r];
-    const float *events = B.events + (size_t) r * B.ev_stride;
     const float source_prob = tb->thresh[0];
-    u64 n_children = 0, n_sources = 0;                 // committed (events confirmed by the tracker)
-    u32 pend_children = 0, pend_sources = 0;           // of the event in flight
     u32 my_blocks = 0, my_steps = 0, pend_blocks = 0, pend_steps = 0;
     u32 prev_size = 0, gen = 0, event_i = n_first;
     if (STREAM) {                                      // resume: the previous chunk's last generation is in the slot
         const DevMapState *ms = B.mstate + B.chan[r];
         if (ms->started) { prev_size = ms->prev_size; gen = ms->gen; }
     }
+    // children / sources of the committed events (confirmed by the tracker): counted by worker thread 0 alone, in
+    // shared memory, so that no thread holds two 64-bit counters through the event loop
+    if (wt == 0) { sh->tot_children[0] = sh->tot_children[1] = 0; sh->tot_sources[0] = sh->tot_sources[1] = 0; }
     const u32 lt = w_lanemask_lt();
-    uint2 *stage_r = (uint2 *) (sh->v2_stage + (size_t) ww * K2V2_STAGE_BYTES);
-    u8 *stage_m = (u8 *) (stage_r + K2_CH_SLOTS);
-    u32 *whist = sh->hist_cur + (size_t) ww * 256u;    // warp-private radix counters (big buckets)
     PT_DECL
     PT_WDECL
 
     for (; event_i < n_limit; event_i++) {
         PT_MARK(9)
-        const float event = f_add(f_mul(scale, events[event_i - n_first]), shift);
+        // (the read's scale, shift and event row are re-read per event: held, they would spill)
+        const float event = f_add(f_mul(B.scale[r], B.events[(size_t) r * B.ev_stride + (event_i - n_first)]), B.shift[r]);
         PT_MARK(7)
 
         // ---- A. pore-model probabilities (reference src/mapper.cpp:443-445); clear the bucket counters
@@ -413,17 +423,20 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
         PT_FENCE
         PT_MARK(16)
 
-        uint4 *prev = W.paths + (size_t) gen * gen_recs * 2, *next = W.paths + (size_t) (gen ^ 1u) * gen_recs * 2;
-        uint2 *hist_e = W.hist + (size_t) (event_i % UNC_NGEN) * gen_recs;
-        const u32 *oprev = W.order + (size_t) gen * maxp;
-        u32 *onext = W.order + (size_t) (gen ^ 1u) * maxp;
-        uint4 *ckA = W.ckey, *ckB = W.ckey + maxp, *cks = W.cks;
-        uint2 *rlist = W.rlist + (size_t) (event_i & 1u) * W.rl_cap;
+        // The event's views of the workspace slot (this generation's records and order, the history ring's slot, the
+        // key arrays, the seed-row buffer) are taken from W (= sh->work) in every phase that uses them: held across
+        // the whole event they do not fit the register budget.
 
         // ---- B. extend every previous path (reference src/mapper.cpp:455-524): chunk c of 32 parents writes its
         //      children, in emission order, to records / keys [c*160, c*160+count)
         const u32 nch_prev = (prev_size + 31u) >> 5;
         {
+            const uint4 *prev = W.paths + (size_t) gen * gen_recs * 2;
+            uint4 *next = W.paths + (size_t) (gen ^ 1u) * gen_recs * 2, *cks = W.cks;
+            uint2 *hist_e = W.hist + (size_t) (event_i % UNC_NGEN) * gen_recs;
+            const u32 *oprev = W.order + (size_t) gen * maxp;
+            uint2 *stage_r = k2v2_stage(sh, ww);
+            u8 *stage_m = (u8 *) (stage_r + K2_CH_SLOTS);
             // software pipeline per warp: the order entry of chunk c+2*nwk is loaded (and its record line requested),
             // the record of chunk c+nwk is loaded (and the Occ block of its row start-1 requested), chunk c is consumed
             u32 oi_n = UNC_INVALID, oi_nn = UNC_INVALID; uint4 q0_n = make_uint4(0, 0, 0, 0); uint2 q1_n = make_uint2(0, 0);   // q1: (seed_prob, C)
@@ -582,6 +595,7 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
             w_sync();
             // seed rows of ended paths, in parent order.  A parent counts only if the buffer was not yet full when
             // the sequential scan reached it (children before it < max_paths).
+            uint2 *rlist = W.rlist + (size_t) (event_i & 1u) * W.rl_cap;
             u32 rows = 0;
             for (u32 i0 = 0; i0 < nch_prev; i0 += 32) {
                 u32 ec = i0 + (u32) lane < nch_prev ? sh->ecnt[i0 + lane] : 0u;
@@ -611,12 +625,20 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
         if (ww != 0 || nwk == 1) {
             const u32 bt = nwk == 1 ? wt : wt - 32u, nbt = nwk == 1 ? nwt : nwt - 32u;
             const u32 nwl = *(volatile u32 *) &sh->wl_cnt;
+            uint4 *next = W.paths + (size_t) (gen ^ 1u) * gen_recs * 2, *cks = W.cks;
+            const uint2 *hist = W.hist;
+            const u32 recs = (u32) gen_recs, s_e = event_i % UNC_NGEN;   // 24 generations of records fit 32-bit offsets
             for (u32 i = bt; i < nwl; i += nbt) {
                 uint4 w = W.wlist[i];
-                u32 idx = w.y;
-                for (u32 j = 1; j <= 21; j++)
-                    idx = W.hist[(size_t) ((event_i + UNC_NGEN - j) % UNC_NGEN) * gen_recs + idx].y;
-                float oldC = u2f(W.hist[(size_t) ((event_i + UNC_NGEN - 22u) % UNC_NGEN) * gen_recs + idx].x);
+                // 21 parent hops back through the history ring, then the C of the ancestor 22 generations back
+                u32 idx = w.y, s = s_e;
+#pragma unroll 1
+                for (u32 j = 0; j < 21u; j++) {
+                    s = s ? s - 1u : UNC_NGEN - 1u;
+                    idx = hist[s * recs + idx].y;
+                }
+                s = s ? s - 1u : UNC_NGEN - 1u;
+                float oldC = u2f(hist[s * recs + idx].x);
                 float sp = f_div(f_sub(u2f(w.z), oldC), 22.0f);
                 uint4 key = cks[w.x];
                 u32 cmc = (u32) d_popc(w.w);
@@ -642,7 +664,7 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
                 const u32 base = sh->bcnt[c], end = c + 1 < nch_prev ? sh->bcnt[c + 1] : nc_total;
                 if (end <= nc) continue;
                 for (u32 i = (base < nc ? nc - base : 0u) + (u32) lane; base + i < end; i += 32)
-                    s_atomic_add(&v2->kagg[v2->t.kslot[cks[(size_t) c * K2_CH_SLOTS + i].w & UNC_KMASK]], 1u);
+                    s_atomic_add(&v2->kagg[v2->t.kslot[W.cks[(size_t) c * K2_CH_SLOTS + i].w & UNC_KMASK]], 1u);
             }
             c_sync_sub(1, (int) nwt);
             if (ww == 0) {
@@ -664,11 +686,13 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
         u32 n_rows = sh->bc[3];
         if (n_rows > W.rl_cap) n_rows = W.rl_cap;
         const u32 n_ended_rows = n_rows;
-        pend_children = nc;
 
         if (nc > 0) {
+          {
             // ---- C1. scatter the keys into their k-mer buckets (any order inside a bucket: the record index is
             //          part of the key); each warp takes the chunks it extended
+            uint4 *ckA = W.ckey;
+            const uint4 *cks = W.cks;
             uint4 kpre = make_uint4(0, 0, 0, 0);                     // the first 32 keys of the warp's next chunk, requested early
             if (ww < nch_prev) {
                 const u32 b0 = sh->bcnt[ww], e0 = ww + 1 < nch_prev ? sh->bcnt[ww + 1] : nc_total;
@@ -692,6 +716,7 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
                     ckA[s_atomic_add(&v2->kcnt[bk], 1u)] = key;
                 }
             }
+          }
             PT_MARK(2)
             c_sync_sub(1, (int) nwt);
             PT_FENCE
@@ -702,6 +727,9 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
             //          group) at a time: first sweep the large buckets (> 32 keys, one warp each, radix), second sweep
             //          the small ones, packed several to a warp pass.
             uint4 *csum = W.elist;                                     // per 32-key chunk of a large bucket: what D1 needs to take it alone
+            uint4 *ckA = W.ckey, *ckB = W.ckey + maxp;
+            uint2 *stage_r = k2v2_stage(sh, ww);
+            u32 *whist = sh->hist_cur + (size_t) ww * 256u;    // warp-private radix counters (big buckets)
             for (;;) {
                 const u32 gi = k2v2_grab(&v2->grab[0]);
                 if (gi >= 96u) break;
@@ -860,6 +888,7 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
         }
         if (ww != 0 || nwk == 1) {
             const u32 bt = nwk == 1 ? wt : wt - 32u, nbt = nwk == 1 ? nwt : nwt - 32u;
+            uint2 *rlist = W.rlist + (size_t) (event_i & 1u) * W.rl_cap;
             for (u32 i = bt; i < n_ended_rows; i += nbt) {
                 uint2 e = rlist[i];
                 e.x = ix.seq_len - unc_sa_lookup(ix, e.x, &pend_steps, &pend_blocks);
@@ -879,7 +908,12 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
         //      handed out through one counter: first the 32-key chunks of the large buckets, one at a time and in any order
         //      (C2 left each chunk its running max and counts), then the groups' merged buckets and packs of small ones.
         if (nc > 0) {
-            const uint4 *csum = W.elist;
+            const uint4 *csum = W.elist, *ckA = W.ckey;
+            uint4 *next = W.paths + (size_t) (gen ^ 1u) * gen_recs * 2;
+            uint2 *hist_e = W.hist + (size_t) (event_i % UNC_NGEN) * gen_recs;
+            u32 *onext = W.order + (size_t) (gen ^ 1u) * maxp;
+            uint2 *rlist = W.rlist + (size_t) (event_i & 1u) * W.rl_cap;
+            uint2 *stage_r = k2v2_stage(sh, ww);
             const u32 n_units = *(volatile u32 *) &v2->n_units;
             for (;;) {
                 const u32 gi = k2v2_grab(&v2->grab[1]);
@@ -982,6 +1016,9 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
         PT_WE(2)
         // ---- E. fresh sources for every sufficiently probable k-mer without one (reference src/mapper.cpp:605-624):
         //      word j (32 k-mers) by warp j % nwk, positions and the buffer-full cut from worker warp 0's plan
+        uint4 *next = W.paths + (size_t) (gen ^ 1u) * gen_recs * 2;
+        uint2 *hist_e = W.hist + (size_t) (event_i % UNC_NGEN) * gen_recs;
+        u32 *onext = W.order + (size_t) (gen ^ 1u) * maxp;
         for (u32 j = ww; j < 32; j += nwk) {
             const u32 before = v2->fresh_before[j];
             if (before >= maxp) continue;                         // never visited: its flags stay as they are
@@ -1020,15 +1057,14 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
         PT_WLAG(0, 13, 14)
         PT_WTRK(3, 25)
         const u32 nn = sh->bc[1];
-        pend_sources = nn - nc;
         const u32 v = event_i > n_first ? *(volatile u32 *) &sh->verdict[(event_i - 1u) & 1u] : 0u;
         if (v) {                                                      // event_i's work is discarded: the Mapper returned
             if (FLAGS && wt < 32u) sh->flags[wt] = sh->flags_prev[wt];   // after event_i - 1 (reference src/mapper.cpp:633-651)
             break;
         }
-        n_children += pend_children; n_sources += pend_sources;
+        if (wt == 0) { k2v2_add64(sh->tot_children, nc); k2v2_add64(sh->tot_sources, nn - nc); }
         my_blocks += pend_blocks; my_steps += pend_steps;
-        pend_children = pend_sources = pend_blocks = pend_steps = 0;
+        pend_blocks = pend_steps = 0;
         prev_size = nn;
         gen ^= 1u;
         PT_MARK(8)
@@ -1037,9 +1073,5 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
     PT_FLUSH(B, r)
     for (int d = 16; d > 0; d >>= 1) { my_blocks += w_shfl(my_blocks, lane ^ d); my_steps += w_shfl(my_steps, lane ^ d); }
     if (lane == 0) { s_atomic_add(&sh->cnt_blocks, my_blocks); s_atomic_add(&sh->cnt_steps, my_steps); }
-    if (wt == 0) {
-        sh->tot_children[0] = (u32) n_children; sh->tot_children[1] = (u32) (n_children >> 32);
-        sh->tot_sources[0] = (u32) n_sources; sh->tot_sources[1] = (u32) (n_sources >> 32);
-    }
     c_sync();                                                         // Y: final barrier
 }
