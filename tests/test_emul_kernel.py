@@ -1,7 +1,7 @@
 """CPU tier: the DEVICE source (uncalled_b200/csrc/unc_device.cuh), compiled for the host with
 -DUNC_EMUL and run under the lockstep CTA emulator (tests/emul/warp_emul.hpp), against the
 oracle.  This exercises the exact kernel logic -- warp scans, the chunk-local extension, the
-segment radix sort, the look-back prefix, the tracker's blocked cluster list -- without a GPU.
+k-mer bucket sort, the bucket-wise dedup walk, the tracker's blocked cluster list -- without a GPU.
 (It is a test vehicle: the shipped library contains only the CUDA build.)"""
 import numpy as np
 import pytest
@@ -65,30 +65,6 @@ def test_full_buffer_semantics(g200k, max_paths):
     _check(E, O, [sig[i] for i in range(4)])
 
 
-@pytest.mark.parametrize("flags,tag", [(("-DK2_LEAN_B", "-DK2_PAR_E"), "_lean_pare"), (("-DK2_TRK_INLINE",), "_trk"),
-                                      (("-DK2_SCAN2", "-DK2_PF2", "-DK2_BMATCH"), "_scan2_pf2_bmatch"),
-                                      (("-DK2_TRK_INLINE", "-DK2_LEAN_B", "-DK2_PAR_E", "-DK2_SCAN2", "-DK2_PF2", "-DK2_DFUSE"), "_all")])
-def test_prototype_variants_keep_parity(g200k, flags, tag):
-    """Compile-time prototypes for a higher-occupancy build must produce the same paths, seeds and PAF records:
-    -DK2_LEAN_B (children written to fixed per-parent slots the moment their base is resolved, Occ words read on
-    demand), -DK2_PAR_E (the fresh-source walk spread over all worker warps with the serial walk's buffer cut) and
-    -DK2_SCAN2 (radix-pass counter scan with one barrier less), -DK2_TRK_INLINE (no dedicated tracker warp: every warp
-    works, worker warp 0 clusters the previous event's seeds in one out-of-line call while the others already extend
-    paths from a dynamic chunk counter), -DK2_PF2 (order entries fetched two chunks ahead of the extension, compaction keys
-    one chunk ahead), -DK2_BMATCH (equal-digit lanes of the radix scatter from eight ballots instead of match.any), -DK2_DFUSE (the k-mer-run
-    aggregates of the dedup phase published inside its main pass: one pass over the keys and one barrier less)."""
-    prefix, g = g200k
-    E = emulib.Emu(prefix, extra_flags=flags, tag=tag)
-    O = orclib.Oracle(prefix)
-    sig, _ = synth.reads(g, 3, 3000, seed=3)
-    _check(E, O, [sig[i] for i in range(2)])
-    _check(E, O, [sig[2]], n_warps=3)
-    if "-DK2_TRK_INLINE" in flags:
-        _check(E, O, [sig[1]], n_warps=1)            # a single warp does everything
-    E.params.max_paths = O.params.max_paths = 300
-    _check(E, O, [sig[i][:2500] for i in range(3)])
-
-
 def test_i16_calibration_path(g200k):
     prefix, g = g200k
     E, O = emulib.Emu(prefix), orclib.Oracle()
@@ -116,7 +92,7 @@ def test_bench_scale_reads_on_the_4m7_index():
 def test_kmer_ranges_that_overlap_share_a_bucket(g200k):
     """get_base_range's start (L2[b], not L2[b]+1) lets a k-mer's FM range begin on its predecessor's last row; children of
     the two k-mers then interleave in the sorted order (first seen on the GPU: read 30 of this set, event 63 -- two gap
-    sources short).  The second worker structure keeps such k-mers in one bucket and walks it as the reference does."""
+    sources short).  The worker warps keep such k-mers in one bucket and walks it as the reference does."""
     prefix, g = g200k
     sig, _ = synth.reads(g, 31, 4000, seed=7)
     E = emulib.Emu(prefix)

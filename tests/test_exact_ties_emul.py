@@ -2,6 +2,7 @@
 uncalled_b200/csrc/unc_pdqsort.cuh) under the emulator, against PAF records computed by the UNMODIFIED reference itself
 (tests/golden/synth_paf_golden.json, tools/make_synth_paf_golden.py) -- including the two reads of that set which the
 reference maps differently from its own stable-sort build -- and against the oracle's restated pdqsort (mode 1)."""
+import ctypes
 import json
 import os
 
@@ -36,11 +37,15 @@ def test_exact_ties_kernel_gives_the_unmodified_references_records(setup):
     assert differ == [64, 137]
     ids = differ + [3, 150]
     sigs = [np.ascontiguousarray(sig[i], np.float32) for i in ids]
+    stats = (ctypes.c_ulong * 2)()
+    E.L.emu_tie_stats(stats, 1)
     try:
         E.set_tie_order(1)
         exact = E.map_batch(sigs)[0]
     finally:
         E.set_tie_order(0)
+    E.L.emu_tie_stats(stats, 1)
+    assert 0 < stats[1] < stats[0], tuple(stats)         # events tested for ties / re-sorted by pdqsort: some, not all
     plain = E.map_batch(sigs)[0]
     O.lib.orc_set_child_sort(1)
     try:
@@ -151,14 +156,13 @@ def test_streaming_path_with_exact_ties(setup):
         O.lib.orc_set_child_sort(0)
 
 
-def test_both_exact_modes_in_the_combined_prototype_build():
-    """The compile-time prototypes of the mapper (no tracker warp, lean extension loop, ...: DESIGN.md section 7) keep the
-    ordered-mode flag handling and the exact-ties sort working -- whichever of them becomes the shipped configuration."""
+def test_ordered_mode_with_exact_ties_on_a_small_buffer_and_a_5_warp_cta():
+    """Ordered mode (sources_added_ carried from read to read) together with exact ties, at max_paths 300 on a 5-warp
+    CTA, against the oracle's pdqsort one-Mapper chain and its flags."""
     import synth
     import synthdata
-    flags = ("-DK2_TRK_INLINE", "-DK2_LEAN_B", "-DK2_PAR_E", "-DK2_SCAN2", "-DK2_PF2", "-DK2_DFUSE")
     prefix, g = synthdata.get_index("g200k")
-    E, O = emulib.Emu(prefix, extra_flags=flags, tag="_all"), orclib.Oracle(prefix)
+    E, O = emulib.Emu(prefix), orclib.Oracle(prefix)
     E.params.max_paths = O.params.max_paths = 300
     sig, _ = synth.reads(g, 40, 2000, seed=21, frac_random=0.4)
     sigs = [np.ascontiguousarray(sig[i], np.float32) for i in (5, 6, 0, 1)]

@@ -1,4 +1,4 @@
-"""CPU sweep of the mapper kernel's second structure (unc_k2v2.cuh) under the emulator: many bench-like reads per
+"""CPU sweep of the mapper kernel's worker warps (unc_k2v2.cuh) under the emulator: many bench-like reads per
 index, PAF fields and the children / sources / seeds / clusters counters against the oracle, in parallel processes.
     python tools/emul_v2_sweep.py <index name> <first read> <n reads> [seed [noise_mult [max_paths [warps per CTA]]]]"""
 import os

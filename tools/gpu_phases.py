@@ -22,24 +22,20 @@ ph2 = np.zeros((n_reads, 64), np.uint64)
 L = N.lib()
 L.unc_pool_debug_phases.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
 N.check(L.unc_pool_debug_phases(bm.h, n_reads, ph2.ctypes.data))
-names = ["A probs", "B extend + B1 deferred seed_prob", "B2 scan/ended rows/key compaction", "C radix sort + fix-up", "D dedup/src", "S sa + E",
-         "X barrier(tracker)", "head: event load + scaling", "head: verdict + bookkeeping", "head: loop back-edge"]
-if os.environ.get("UNC_PHASES_V1") is None:     # the second worker structure (unc_k2v2.cuh) marks its own phases
-    names = ["A probs + counter reset", "B extension", "C1 scatter into k-mer buckets", "C2 bucket sort + count", "(unused)", "D1 dedup/sources/seeds + E fresh",
-             "X barrier wait (slowest warp of D1/E, tracker)", "head: event load + scaling", "head: verdict + bookkeeping", "head: loop back-edge",
-             "B2 chunk scan / ended rows / bucket offsets / deferred seed_prob", "D0 bucket prefix + flags + fresh plan | S1 SA of ended rows",
-             "cut-case recount", "", "", "",
-             "  wait at the barrier after A", "  wait after B", "  wait after C1", "  wait after C2", "", "", "", "", "", "", "  wait after B2", "  wait after D0", "", "", "", ""]
+names = ["A probs + counter reset", "B extension", "C1 scatter into k-mer buckets", "C2 bucket sort + count", "(unused)", "D1 dedup/sources/seeds + E fresh",
+         "X barrier wait (slowest warp of D1/E, tracker)", "head: event load + scaling", "head: verdict + bookkeeping", "head: loop back-edge",
+         "B2 chunk scan / ended rows / bucket offsets / deferred seed_prob", "D0 bucket prefix + flags + fresh plan | S1 SA of ended rows",
+         "cut-case recount", "", "", "",
+         "  wait at the barrier after A", "  wait after B", "  wait after C1", "  wait after C2", "", "", "", "", "", "", "  wait after B2", "  wait after D0", "", "", "", ""]
 ev = out["events_used"].astype(np.float64) + 1
 for title, ph in (("worker warp 0, thread 0 (also runs the single-warp sections)", ph2[:, :32]),
                   ("last worker warp, lane 0 (its barrier waits expose the single-warp sections)", ph2[:, 32:64])):
     tot = ph.sum(axis=0).astype(np.float64)
     per_warp = tot.copy()
-    if os.environ.get("UNC_PHASES_V1") is None:
-        tot[[13, 14, 15, 20, 21, 22, 23, 24, 25]] = 0      # not intervals: the worker warps' own times (slowest / mean), below
-        ph = ph.copy(); ph[:, [13, 14, 15, 20, 21, 22, 23, 24, 25]] = 0
-        if title.startswith("last"):
-            ph[:, 28:32] = 0; tot[28:32] = 0           # the tracker's counters
+    tot[[13, 14, 15, 20, 21, 22, 23, 24, 25]] = 0      # not intervals: the worker warps' own times (slowest / mean), below
+    ph = ph.copy(); ph[:, [13, 14, 15, 20, 21, 22, 23, 24, 25]] = 0
+    if title.startswith("last"):
+        ph[:, 28:32] = 0; tot[28:32] = 0           # the tracker's counters
     print("--", title)
     print("total events", ev.sum())
     for i, nm in enumerate(names):
@@ -47,7 +43,7 @@ for title, ph in (("worker warp 0, thread 0 (also runs the single-warp sections)
             continue
         print("%-36s %6.1f%%  %8.0f cycles/event" % (nm, 100 * tot[i] / max(tot.sum(), 1), tot[i] / ev.sum()))
     print("cycles/event total %.0f" % (tot.sum() / ev.sum()))
-    if os.environ.get("UNC_PHASES_V1") is None and title.startswith("worker"):
+    if title.startswith("worker"):
         print("   event barrier: now - release stamp of the last-released worker warp %.0f, of the first-released %.0f" % (per_warp[13] / ev.sum(), per_warp[14] / ev.sum()))
         for nm, a, b in (("C2 sort + count", 15, 20), ("D1 emit", 21, 22)):
             print("   %-18s slowest worker warp %8.0f cycles/event, mean warp %8.0f" % (nm, per_warp[a] / ev.sum(), per_warp[b] / ev.sum()))

@@ -1,7 +1,7 @@
 """Register / spill report of the mapper kernels, from the compiler alone (no GPU needed).
 
 Compiles uncalled_b200/csrc/unc_abi.cu for sm_90a with the library's own nvcc flags plus -Xptxas -v, then prints for
-k2_map, k2_map_ord and k2_map_stream:
+k2_map, k2_map_ord, k2_map_stream and the exact-ties kernels k2_map_exact and k2_map_stream_exact:
   * registers, stack frame and spill bytes as ptxas reports them;
   * the local-memory instructions (LDL / STL) of the kernel's SASS per source line, from `nvdisasm -g` on the cubin
     (inlined code is attributed to the line of the inlined function, which is where the spill sits).
@@ -13,7 +13,7 @@ import argparse, collections, os, re, subprocess, sys, tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "uncalled_b200", "csrc", "unc_abi.cu")
-KERNELS = ("k2_map", "k2_map_ord", "k2_map_stream")
+KERNELS = ("k2_map", "k2_map_ord", "k2_map_stream", "k2_map_exact", "k2_map_stream_exact")
 
 
 def nvcc_flags():
@@ -43,7 +43,7 @@ def demangled_name(mangled):
 
 def ptxas_stats(text):
     """{kernel: {"regs", "stack", "spill_st", "spill_ld"}} from `ptxas -v` output"""
-    res, cur = {}, None
+    res, cur, props = {}, None, None
     for l in text.split("\n"):
         m = re.search(r"Compiling entry function '(\S+)'", l)
         if m:
@@ -52,8 +52,12 @@ def ptxas_stats(text):
             continue
         if cur is None:
             continue
+        m = re.search(r"Function properties for (\S+)", l)
+        if m:                                          # the kernel's own, or those of a non-inlined callee (unc_pdq_sort)
+            props = demangled_name(m.group(1))
+            continue
         m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", l)
-        if m:
+        if m and props == cur:
             res[cur].update(stack=int(m.group(1)), spill_st=int(m.group(2)), spill_ld=int(m.group(3)))
         m = re.search(r"Used (\d+) registers", l)
         if m:
@@ -86,10 +90,10 @@ def spill_lines(cubin, kernels=KERNELS):
 
 
 def report(stats, lines, kernels=KERNELS):
-    print("%-14s %5s %6s %9s %9s %6s %6s" % ("kernel", "regs", "stack", "spill_st", "spill_ld", "LDL", "STL"))
+    print("%-20s %5s %6s %9s %9s %6s %6s" % ("kernel", "regs", "stack", "spill_st", "spill_ld", "LDL", "STL"))
     for k in kernels:
         s, ln = stats.get(k, {}), lines.get(k, {})
-        print("%-14s %5s %6s %9s %9s %6d %6d" % (k, s.get("regs"), s.get("stack"), s.get("spill_st"), s.get("spill_ld"),
+        print("%-20s %5s %6s %9s %9s %6d %6d" % (k, s.get("regs"), s.get("stack"), s.get("spill_st"), s.get("spill_ld"),
                                                  sum(v[0] for v in ln.values()), sum(v[1] for v in ln.values())))
     for k in kernels:
         ln = lines.get(k, {})

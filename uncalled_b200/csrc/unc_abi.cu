@@ -31,13 +31,8 @@ static_assert(sizeof(DevReadDesc) == 32, "DevReadDesc layout");
 #define K2_MIN_CTAS 2       /* 2 CTAs x 14 warps per SM (72 registers): on an H100 SXM (400 W limit) 4 510 reads/s on the
                                bench workload, against 4 230 for 2 x 8 warps, 4 200 for 1 x 16 and 3 960 for 1 x 14 */
 #endif
-#define K2_MIN_CTAS_V1 (K2_WARPS > 8 ? 1 : 2)    /* first structure (exact-ties kernels): 127 registers */
 #define K2_THREADS (K2_WARPS * 32)
-#ifdef K2_TRK_INLINE
-static_assert(K2_WARPS >= 1 && K2_WARPS <= K2_MAXSEG, "worker warps (all of them) must fit the sort segments");
-#else
-static_assert(K2_WARPS >= 2 && K2_WARPS - 1 <= K2_MAXSEG, "worker warps must fit the sort segments");
-#endif
+static_assert(K2_WARPS >= 2 && K2_WARPS - 1 <= K2_MAXSEG, "worker warps must fit the per-warp shared-memory arrays");
 
 __global__ void k_kmer_ranges(DevIndex ix, uint2 *out) {
     u32 k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -86,7 +81,7 @@ __global__ void __launch_bounds__(128) k1_norm(DevBatch B, DevParams p) {
 // and the thresholds in shared memory, then pulls reads from a global queue; the K2_WARPS warps
 // of the CTA cooperate on every event of the read (chained scans through shared memory).
 #define K2_MAP_KERNEL(NAME, EXACT, FLAGS)                                                                                       \
-    __global__ void __launch_bounds__(K2_THREADS, (EXACT) ? K2_MIN_CTAS_V1 : K2_MIN_CTAS)                                  \
+    __global__ void __launch_bounds__(K2_THREADS, K2_MIN_CTAS)                                                             \
     NAME(DevIndex ix, DevParams p, DevBatch B, DevWork W0, size_t paths_stride, size_t hist_stride, size_t ckey_stride,     \
          size_t cks_stride, size_t elist_stride, size_t order_stride, size_t rlist_stride, size_t clu_stride,              \
          size_t dir_stride) {                                                                                              \
@@ -357,7 +352,7 @@ int unc_index_load(const char *bwa_prefix, const char *preset, const char *model
     x->kmer_range.resize(1024);
     cudaError_t e = cudaMemcpy(x->kmer_range.data(), x->d_kr, 1024 * sizeof(uint2), cudaMemcpyDeviceToHost);
     if (e != cudaSuccess) { unc_index_free(x); return fail(UNC_E_CUDA, std::string("k_kmer_ranges: ") + cudaGetErrorString(e)); }
-    {   // GPU-side layouts of the mapper's second structure: 32-byte Occ blocks, k-mer rank tables
+    {   // GPU-side layouts of the mapper's worker warps: 32-byte Occ blocks, k-mer rank tables
         const u32 n_blk = (u32) (h.bwt.size() / 16) * 2u;
         if (cudaMalloc(&x->d_occ2, (size_t) n_blk * 32 + 64) != cudaSuccess) { unc_index_free(x); return fail(UNC_E_CUDA, "cudaMalloc occ2"); }
         cudaMemset((char *) x->d_occ2 + (size_t) n_blk * 32, 0, 64);
@@ -732,8 +727,6 @@ int unc_pool_set_tie_order(unc_pool *P, int mode) {
     if (mode == 1) {
         CUDA_TRY(cudaSetDevice(P->idx->device));
         CUDA_TRY(raise_dyn_smem(k2_map_exact, P->smem));
-        // CTAs are independent (each pulls reads from the queue into its own slot), so a lower residency than k2_map's
-        // only means that the last CTAs of the grid start late and find the queue empty
     }
     P->tie_order = mode;
     return UNC_OK;
