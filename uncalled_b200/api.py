@@ -64,6 +64,15 @@ class Conf:
         "ordered": (0, "1: map the reads in input order as ONE long-lived Mapper does, i.e. exactly what the reference "
                        "prints with `-t 1` (a read inherits the source flags its predecessor left set); "
                        "0: every read is mapped by a new Mapper (batch order free, fastest)"),
+        # read-until simulator (`uncalled sim`); defaults: the [simulator] section of the reference's conf/defaults.toml
+        "ctl_seqsum": ("", "Sequencing summary of the control run whose reads are replayed"),
+        "unc_seqsum": ("", "Sequencing summary of the UNCALLED run that gives the channel activity pattern"),
+        "unc_paf": ("", "PAF of the UNCALLED run (its ej/ub tags give the eject delay)"),
+        "sim_speed": (1.0, "Scale factor applied to the scan interval boundaries"),
+        "scan_time": (10.0, "Length of a simulated mux scan in seconds"),
+        "scan_intv_time": (5400.0, "Time between mux scans in seconds"),
+        "ej_time": (0.1, "Extra gap after an ejected read in seconds"),
+        "min_ch_reads": (10, "Minimum number of control reads given to a channel that had reads in the UNCALLED run"),
     }
 
     def __init__(self):
@@ -412,10 +421,18 @@ class MapPool:
 
 
 class Chunk:
-    """reference src/chunk.hpp:33-81 (the vector<float> constructor form and the accessors pybind exports)."""
+    """reference src/chunk.hpp:33-81 (the vector<float> constructor form and the accessors pybind exports).
+    With `calibration=(range, offset, digitisation)` the samples are int16 DAC values, kept as they are and
+    calibrated on the device when RealtimePool maps them."""
 
-    def __init__(self, read_id="", channel=1, number=0, start=0, raw_data=(), raw_st=0, raw_len=None):
-        raw = np.asarray(raw_data, dtype=np.float32)
+    def __init__(self, read_id="", channel=1, number=0, start=0, raw_data=(), raw_st=0, raw_len=None, calibration=None):
+        if calibration is None:
+            raw, self.dtype, self.cal = np.asarray(raw_data, dtype=np.float32), 0, (1.0, 0.0, 1.0)
+        else:
+            raw = np.asarray(raw_data)
+            if raw.dtype != np.int16:
+                raise TypeError("calibration given: the samples must be int16 DAC values")
+            self.dtype, self.cal = 1, tuple(float(np.float32(x)) for x in calibration)
         if raw_len is None:
             raw_len = len(raw) - raw_st
         if raw_st + raw_len > len(raw):                   # Chunk::Chunk clips to the signal (src/chunk.cpp:74-83)
@@ -430,7 +447,7 @@ class Chunk:
         return len(self._raw) == 0
 
     def pop(self):
-        r, self._raw = self._raw, np.zeros(0, np.float32)
+        r, self._raw = self._raw, np.zeros(0, self._raw.dtype)
         return r
 
     def swap(self, other):
@@ -520,11 +537,13 @@ class RealtimePool:
         if self._stopped:
             return []
         out = []
-        for phase in (0, 1):                # phase 0: resets of reads in progress; phase 1: the buffered chunks
+        # phase 0: resets of reads in progress; phase 1: the buffered chunks, float32 ones first and then int16
+        # ones (a step carries one sample type)
+        for phase, dtype in ((0, 0), (1, 0), (1, 1)):
             descs, parts, chans, off = [], [], [], 0
             for ch in range(self.conf.num_channels):
                 d = S.ChunkDesc()
-                d.channel, d.dtype = ch, 0
+                d.channel, d.dtype = ch, dtype
                 d.cal_range, d.cal_offset, d.cal_digit = 1.0, 0.0, 1.0
                 if phase == 0:
                     if not (self._reset[ch] and self._active(ch)):
@@ -532,8 +551,9 @@ class RealtimePool:
                     d.new_read, d.offset, d.n_samples = 0, 0, 0
                 else:
                     c = self._pending[ch]
-                    if c is None:
+                    if c is None or c.dtype != dtype:
                         continue
+                    d.cal_range, d.cal_offset, d.cal_digit = c.cal
                     raw = c.pop()
                     d.new_read, d.offset, d.n_samples = (1 if self._fresh[ch] else 0), off, len(raw)
                     if self._fresh[ch]:
@@ -546,7 +566,7 @@ class RealtimePool:
             if not descs:
                 continue
             arr = (S.ChunkDesc * len(descs))(*descs)
-            flat = np.concatenate(parts) if parts else np.zeros(1, np.float32)
+            flat = np.concatenate(parts) if parts else np.zeros(1, np.float32 if dtype == 0 else np.int16)
             res = (S.StreamResult * len(descs))()
             self.backend.step(arr, len(descs), flat, res)
             for ch, r in zip(chans, res):

@@ -1,4 +1,4 @@
-"""`uncalled index` and `uncalled map` (reference scripts/uncalled:38-78,127-167 with the options of
+"""`uncalled index`, `uncalled map` and `uncalled sim` (reference scripts/uncalled:38-78,127-167 with the options of
 uncalled/args.py:87-161,218-286) on this package: same sub-commands, option names, defaults, stderr progress
 lines and PAF output.  `python -m uncalled_b200 map <prefix> <fast5s...>`.  `--device` picks the GPU of this
 process; under `torchrun --nproc-per-node N -m uncalled_b200 map ...` every rank maps its share of the fast5 files on
@@ -51,6 +51,36 @@ def get_parser(conf):
     p.add_argument("--batch-reads", type=int, default=conf.batch_reads, help="Reads per GPU batch")
     p.add_argument("--ordered", action="store_const", const=1, default=conf.ordered, help=type(conf).ordered.__doc__)
     p.add_argument("--exact-ties", action="store_const", const=1, default=conf.exact_ties, help=type(conf).exact_ties.__doc__)
+
+    p = sp.add_parser("sim", help="Simulate real-time targeted sequencing (read until) from a control run and an "
+                      "UNCALLED run", formatter_class=fmt)
+    p.add_argument("bwa_prefix", type=str, help="BWA prefix to mapping to. Must be processed by \"uncalled index\".")
+    p.add_argument("-p", "--idx-preset", type=str, default=conf.idx_preset, help="Mapping mode")
+    p.add_argument("fast5s", nargs="+", type=str, help="Reads of the control run. Can be a directory which will be "
+                   "recursively searched for all files with the \".fast5\" extension, a text file containing one fast5 "
+                   "filename per line, or a comma-separated list of fast5 file names.")
+    p.add_argument("-r", "--recursive", action="store_true")
+    p.add_argument("--ctl-seqsum", type=str, required=True, help=type(conf).ctl_seqsum.__doc__)
+    p.add_argument("--unc-seqsum", type=str, required=True, help=type(conf).unc_seqsum.__doc__)
+    p.add_argument("--unc-paf", type=str, required=True, help=type(conf).unc_paf.__doc__)
+    p.add_argument("--sim-speed", type=float, default=conf.sim_speed, help=type(conf).sim_speed.__doc__)
+    p.add_argument("-t", "--threads", type=int, default=conf.threads, help="Number of host threads (fast5 decoding; the mapping runs on the GPU)")
+    p.add_argument("--num-channels", type=int, default=conf.num_channels, help="Number of channels used in sequencing.")
+    p.add_argument("-e", "--max-events", type=int, default=conf.max_events, help="Will give up on a read after this many events have been processed")
+    p.add_argument("-c", "--max-chunks", type=int, default=conf.max_chunks, help="Will give up on a read after this many chunks have been processed.")
+    p.add_argument("--chunk-time", type=float, default=1, required=False, help="Length of chunks in seconds")
+    p.add_argument("--exact-ties", action="store_const", const=1, default=conf.exact_ties, help=type(conf).exact_ties.__doc__)
+    from .api import RealtimePool as RP
+    modes = p.add_mutually_exclusive_group(required=True)          # uncalled/args.py:161-188
+    modes.add_argument("-D", "--deplete", action="store_const", const=RP.DEPLETE, dest="realtime_mode",
+                       help="Will eject reads that align to index")
+    modes.add_argument("-E", "--enrich", action="store_const", const=RP.ENRICH, dest="realtime_mode",
+                       help="Will eject reads that don't align to index")
+    active = p.add_mutually_exclusive_group()
+    active.add_argument("--full", action="store_const", const=RP.FULL, dest="active_chs", help="Will monitor all pores if set (default)")
+    active.add_argument("--even", action="store_const", const=RP.EVEN, dest="active_chs", help="Will only monitor even pores if set")
+    active.add_argument("--odd", action="store_const", const=RP.ODD, dest="active_chs", help="Will only monitor odd pores if set")
+    p.add_argument("--device", type=int, default=conf.device, help="CUDA device")
 
     p = sp.add_parser("mask-internal", help="Iteratively masks the most frequent k-mer of a FASTA reference with N "
                       "(masking/mask_internal.sh)", formatter_class=fmt)
@@ -147,6 +177,21 @@ def map_cmd(conf, args, out=None):
     mapper.stop()
 
 
+def sim_cmd(conf, args, out=None):
+    """scripts/uncalled:169-300 with `sim`: the pattern and the control reads are loaded, then the decision loop runs
+    until every simulated channel has run out.  Bad input ends the command with status 1 before the GPU is touched."""
+    from .sim import SimError, run_sim
+    assert_exists(conf.bwa_prefix + ".bwt")
+    assert_exists(conf.bwa_prefix + ".uncl")
+    files = [f for f in load_fast5s(args.fast5s, args.recursive) if f is not None]
+    try:
+        run_sim(conf, files, out)
+    except SimError as e:
+        sys.stderr.write("Error: %s\n" % e)
+        sys.exit(1)
+    sys.stderr.write("Finished\n")
+
+
 def load_conf(argv):
     """uncalled/args.py:288-302: every parsed option whose name is a Conf attribute is set on the Conf."""
     from .api import Conf
@@ -165,6 +210,8 @@ def main(argv=None):
         index_cmd(args)
     elif args.subcmd == "map":
         map_cmd(conf, args)
+    elif args.subcmd == "sim":
+        sim_cmd(conf, args)
     elif args.subcmd == "mask-internal":
         from . import _native as N
         from .mask import mask_internal
