@@ -316,6 +316,32 @@ int unc_mask_internal(const char *fasta_in, const char *out_fasta, uint32_t k, u
                       uint64_t *counts, uint32_t *n_done);
 float unc_mask_last_kernel_ms(void);
 
+/* ---- external repeat masking of a target against a full reference (`mask-external`) ----------------------------
+ *   unc_mask_external   masking/mask_external.sh <full_bowtie> <target_fa> <min_len> <min_copy> <threads> <out_prefix>:
+ *                       every full-length window of min_len bases of every target record (`bedtools makewindows -s 1`),
+ *                       its exact hits on both strands of the full reference (`bowtie -fa -v 0`), the union of the
+ *                       windows with more than min_copy hits masked (`bedtools merge` + `maskfasta`)
+ * Both FASTA files are read as unc_mask_internal reads them.  A window's count is occ(w) + occ(revcomp(w)) over the
+ * forward text of every full-reference record: bases are case-insensitive, any other byte and a record boundary break
+ * an occurrence, a palindrome counts 2 per locus, counts saturate at UINT32_MAX.  A window with a non-ACGT byte has
+ * count 0.  out_fasta: each stripped header, then the sequence on one line with the masked positions as 'N' and every
+ * other byte as in the input.  out_bed: `name\tstart\tend` per maximal run of masked positions (0-based, half-open,
+ * name = the header's first word), in record order.  window_counts (optional, one per target position in the order of
+ * the records, one more between records): the count of the window starting there, 0 where none starts.  The full
+ * reference is streamed through the device in pieces of piece_bases window starts (0 = 64 Mi), so device memory is
+ * the target's table plus two pieces.  UNC_E_ARG (nothing written) for min_len outside 2..64, min_copy < 1, a missing
+ * output directory, or either FASTA empty, not starting with '>' or with a record without sequence; UNC_E_TOO_LARGE
+ * for 2^32 or more bases in either file.
+ * unc_mask_external_last_kernel_ms: CUDA-event time of the last call's kernels.  unc_mask_external_last_times:
+ * ms[0..3] = build, count (summed over the pieces), mark, and the count phase from the end of the build to the end of
+ * the last count kernel (the part of it not spent in count kernels is copying and staging that was not hidden);
+ * *h2d_bytes = the bytes copied to the device. */
+int unc_mask_external(const char *full_fasta, const char *target_fasta, uint32_t min_len, uint32_t min_copy,
+                      const char *out_fasta, const char *out_bed, uint64_t piece_bases, uint32_t *window_counts,
+                      uint64_t *n_selected, uint64_t *n_masked_bp);
+float unc_mask_external_last_kernel_ms(void);
+void unc_mask_external_last_times(float ms[4], uint64_t *h2d_bytes);
+
 /* ---- fast5 input (host; no libhdf5 needed) -------------------------------------------------------------
  *   unc_fast5_open      Fast5Reader::open_next: format detection and the list of reads
  *                                                      src/fast5_reader.cpp:134-177

@@ -85,7 +85,8 @@ EXPORTS = ["unc_strerror", "unc_last_error", "unc_device_count", "unc_init", "un
            "unc_fm_sa", "unc_pool_last_timing", "unc_pool_k1_stats", "unc_stream_create", "unc_stream_set_tie_order", "unc_stream_set_chunk_timeout", "unc_stream_last_step_ms", "unc_stream_step",
            "unc_stream_free", "unc_self_align", "unc_free", "unc_fast5_open", "unc_fast5_count", "unc_fast5_info",
            "unc_fast5_load", "unc_fast5_close", "unc_fast5_last_error", "unc_dtw_batch", "unc_dtw_release", "unc_dtw_last_kernel_ms",
-           "unc_mask_internal", "unc_mask_last_kernel_ms"]
+           "unc_mask_internal", "unc_mask_last_kernel_ms", "unc_mask_external", "unc_mask_external_last_kernel_ms",
+           "unc_mask_external_last_times"]
 
 
 def build(force=False, verbose=False):
@@ -96,6 +97,7 @@ def build(force=False, verbose=False):
                    ("unc_device.cuh", "unc_k2v2.cuh", "unc_dtw.cuh", "unc_dtw_host.inl", "unc_k1.cuh", "unc_stream.cuh", "unc_stream_host.inl", "unc_stream_logic.hpp", "unc_ordered_logic.hpp", "unc_pdqsort.cuh", "unc_warp.cuh",
                     "unc_selfalign.cuh", "unc_selfalign_host.hpp", "unc_selfalign_host.inl",
                     "unc_mask.cuh", "unc_mask_host.hpp", "unc_mask_host.inl",
+                    "unc_mask_ext.cuh", "unc_mask_ext_host.hpp", "unc_mask_ext_host.inl",
                     "unc_host_index.hpp", "unc_host_params.hpp")] + \
         [os.path.join(ROOT, "include", "unc_b200.h")]
     if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps):
@@ -191,6 +193,12 @@ def lib():
     L.unc_mask_internal.argtypes = [C.c_char_p, C.c_char_p, u32, u32, vp, vp, C.POINTER(u32)]
     L.unc_mask_last_kernel_ms.argtypes = []
     L.unc_mask_last_kernel_ms.restype = C.c_float
+    L.unc_mask_external.argtypes = [C.c_char_p, C.c_char_p, u32, u32, C.c_char_p, C.c_char_p, u64, vp, C.POINTER(u64),
+                                    C.POINTER(u64)]
+    L.unc_mask_external_last_kernel_ms.argtypes = []
+    L.unc_mask_external_last_kernel_ms.restype = C.c_float
+    L.unc_mask_external_last_times.argtypes = [vp, C.POINTER(u64)]
+    L.unc_mask_external_last_times.restype = None
     _lib = L
     return L
 

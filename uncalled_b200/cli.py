@@ -90,6 +90,16 @@ def get_parser(conf):
     p.add_argument("out_prefix", type=str, help="output prefix: writes <out_prefix>mask<iters>.fa")
     p.add_argument("--device", type=int, default=0, help="CUDA device")
 
+    p = sp.add_parser("mask-external", help="Masks the windows of a target reference that occur more than min_copy "
+                      "times in a full reference, on either strand (masking/mask_external.sh)", formatter_class=fmt)
+    p.add_argument("full_reference", type=str, help="fasta file of the full reference (e.g. the whole genome)")
+    p.add_argument("target", type=str, help="fasta file of the target reference to mask")
+    p.add_argument("min_len", type=int, help="window length (2 to 64)")
+    p.add_argument("min_copy", type=int, help="windows with more than this many copies are masked")
+    p.add_argument("out_prefix", type=str, help="output prefix: writes <out_prefix>masked<min_copy>.fa and "
+                   "<out_prefix>reps_m<min_copy>.bed")
+    p.add_argument("--device", type=int, default=0, help="CUDA device")
+
     p = sp.add_parser("pafstats",help="Computes speed and accuracy of UNCALLED mappings.", formatter_class=fmt)
     p.add_argument("infile", type=str, help="PAF file output by UNCALLED")          # uncalled/pafstats.py:165-169
     p.add_argument("-n", "--max-reads", required=False, type=int, default=None, help="Will only look at first n reads if specified")
@@ -220,6 +230,14 @@ def main(argv=None):
         done = mask_internal(args.reference, args.k, args.iters, args.out_prefix)
         if len(done) < args.iters:
             sys.stderr.write("No k-mer left to mask after %d iterations\n" % len(done))
+    elif args.subcmd == "mask-external":
+        from . import _native as N
+        from .mask import mask_external
+        assert_exists(args.full_reference)
+        assert_exists(args.target)
+        N.check(N.lib().unc_init(args.device))
+        masked, _ = mask_external(args.full_reference, args.target, args.min_len, args.min_copy, args.out_prefix)
+        sys.stdout.write("Masked %d basepairs\n" % masked)
     elif args.subcmd == "pafstats":
         from . import pafstats
         pafstats.run(args.infile, args.ref_paf, args.max_reads)

@@ -36,6 +36,10 @@ UNC_DEV uint32_t w_shfl_down(uint32_t v, int d) { return __shfl_down_sync(UNC_FU
 UNC_DEV uint32_t w_match(uint32_t v) { return __match_any_sync(UNC_FULL, v); }
 UNC_DEV uint32_t d_atomic_add(uint32_t *p, uint32_t v) { return atomicAdd(p, v); }
 UNC_DEV uint32_t d_atomic_or(uint32_t *p, uint32_t v) { return atomicOr(p, v); }
+// 16-byte compare-and-swap on global memory (sm_90: ATOMG.E.CAS.128); p 16-byte aligned
+UNC_DEV unsigned __int128 d_atomic_cas128(unsigned __int128 *p, unsigned __int128 cmp, unsigned __int128 v) {
+    return atomicCAS(p, cmp, v);
+}
 UNC_DEV uint32_t s_atomic_add(uint32_t *p, uint32_t v) { return atomicAdd(p, v); }
 UNC_DEV uint32_t s_atomic_or(uint32_t *p, uint32_t v) { return atomicOr(p, v); }
 UNC_DEV uint32_t s_atomic_max(uint32_t *p, uint32_t v) { return atomicMax(p, v); }
