@@ -13,6 +13,7 @@
  *                       BwaIndex::load_index           src/bwa_index.hpp:116-135
  *   unc_index_build     BwaIndex::create -> bwa_idx_build
  *                                                      src/bwa_index.hpp:92-101
+ *   unc_index_build_device  the same files, built on the GPU
  *   unc_params_default  Mapper::PRMS and sub-structs   src/mapper.cpp:29-52,
  *                       seed_tracker.cpp:28-32, event_detector.cpp:17-26,
  *                       read_buffer.cpp:26-32          (what Conf binds, src/conf.hpp:57-95)
@@ -145,8 +146,21 @@ int unc_index_kmer_range(const unc_index *idx, uint32_t kmer, uint64_t *start, u
 int unc_index_thresholds(const unc_index *idx, float out[64]);
 void unc_index_free(unc_index *idx);
 
-/* bwa-compatible FM-index construction (.pac .ann .amb .bwt .sa), host C++. */
+/* bwa-compatible FM-index construction (.pac .ann .amb .bwt .sa), host C++.  UNC_E_TOO_LARGE when 2 x the
+ * reference length + 1 reaches 0x7FFFFFF0 (its suffix array is int32). */
 int unc_index_build(const char *fasta_path, const char *prefix);
+/* The same five files, byte for byte, with the suffix sort and the BWT / Occ / SA construction on the device selected
+ * by unc_init.  Accepts every reference whose seq_len = 2 x length is below 0xFFFFFF00 (what unc_index_load accepts):
+ * UNC_E_TOO_LARGE above, UNC_E_NO_DEVICE without a device, UNC_E_NOMEM when the device's free memory is below what
+ * the build needs; in each of these cases nothing is written.  Device memory: at most 16.4 bytes per FM row plus a sort
+ * workspace (DESIGN.md section 4, "FM-index build").
+ * unc_index_build_device_last_times: CUDA-event time of the last successful call's phases, ms[0..2] = initial sort
+ * (with the upload of the text), doubling rounds, BWT / Occ / SA output (with the copy back); *rounds = doubling rounds;
+ * *peak_bytes = the most device memory the build held at once.  unc_index_build_device_last_active: the active rows
+ * (rows of groups not yet sorted) of each doubling round, up to cap of them; returns the number of rounds. */
+int unc_index_build_device(const char *fasta_path, const char *prefix);
+void unc_index_build_device_last_times(float ms[3], uint32_t *rounds, uint64_t *peak_bytes);
+uint32_t unc_index_build_device_last_active(uint64_t *active, uint32_t cap);
 
 /* Device workspace for batches of at most max_reads reads / max_samples samples in total. */
 int unc_pool_create(const unc_index *idx, const unc_params *prm, uint32_t max_reads,

@@ -86,7 +86,8 @@ EXPORTS = ["unc_strerror", "unc_last_error", "unc_device_count", "unc_init", "un
            "unc_stream_free", "unc_self_align", "unc_free", "unc_fast5_open", "unc_fast5_count", "unc_fast5_info",
            "unc_fast5_load", "unc_fast5_close", "unc_fast5_last_error", "unc_dtw_batch", "unc_dtw_release", "unc_dtw_last_kernel_ms",
            "unc_mask_internal", "unc_mask_last_kernel_ms", "unc_mask_external", "unc_mask_external_last_kernel_ms",
-           "unc_mask_external_last_times"]
+           "unc_mask_external_last_times", "unc_index_build_device", "unc_index_build_device_last_times",
+           "unc_index_build_device_last_active"]
 
 
 def build(force=False, verbose=False):
@@ -98,6 +99,7 @@ def build(force=False, verbose=False):
                     "unc_selfalign.cuh", "unc_selfalign_host.hpp", "unc_selfalign_host.inl",
                     "unc_mask.cuh", "unc_mask_host.hpp", "unc_mask_host.inl",
                     "unc_mask_ext.cuh", "unc_mask_ext_host.hpp", "unc_mask_ext_host.inl",
+                    "unc_fmb.cuh", "unc_fmb_run.hpp", "unc_fmb_host.inl", "unc_index_host.hpp",
                     "unc_host_index.hpp", "unc_host_params.hpp")] + \
         [os.path.join(ROOT, "include", "unc_b200.h")]
     if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps):
@@ -155,6 +157,11 @@ def lib():
     L.unc_index_free.argtypes = [vp]
     L.unc_index_free.restype = None
     L.unc_index_build.argtypes = [C.c_char_p, C.c_char_p]
+    L.unc_index_build_device.argtypes = [C.c_char_p, C.c_char_p]
+    L.unc_index_build_device_last_times.argtypes = [C.POINTER(C.c_float), C.POINTER(u32), C.POINTER(u64)]
+    L.unc_index_build_device_last_times.restype = None
+    L.unc_index_build_device_last_active.argtypes = [C.POINTER(u64), u32]
+    L.unc_index_build_device_last_active.restype = u32
     L.unc_pool_create.argtypes = [vp, C.POINTER(Params), u32, u64, C.POINTER(vp)]
     L.unc_pool_free.argtypes = [vp]
     L.unc_pool_free.restype = None

@@ -370,7 +370,9 @@ class RealtimePool {
 // ------------------------------------------------------------------ index side
 struct BwaIndex {
     static void create(const std::string &fasta, const std::string &prefix) {        // BwaIndex::create, src/bwa_index.hpp:92-101
-        check(unc_index_build(fasta.c_str(), prefix.c_str()), "unc_index_build");
+        // the device builder where a CUDA device is visible; both write the same files
+        if (unc_device_count() > 0) check(unc_index_build_device(fasta.c_str(), prefix.c_str()), "unc_index_build_device");
+        else check(unc_index_build(fasta.c_str(), prefix.c_str()), "unc_index_build");
     }
 };
 static std::vector<std::vector<u64>> self_align(const std::string &prefix, u32 sample_dist) {   // src/self_align_ref.cpp:34-91

@@ -11,6 +11,8 @@
 // The BWT is a mathematical object, so it is built here with a linear-time SA-IS suffix
 // sorter written for this project rather than with bwa's is.c / bwt_gen.c.
 // Ambiguous bases become lrand48()&3 after srand48(11) exactly as bwa does (bntseq.c:266,296).
+// The host steps (FASTA, .pac/.ann/.amb, the .bwt/.sa layout) are unc_index_host.hpp's, shared with the device
+// builder unc_index_build_device (unc_fmb_host.inl); this file's own part is the suffix sort and the BWT / Occ / SA.
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -18,7 +20,7 @@
 #include <string>
 #include <vector>
 
-#include "../../include/unc_b200.h"
+#include "unc_index_host.hpp"
 
 namespace {
 
@@ -92,117 +94,19 @@ void sais(const T *s, int32_t *SA, int32_t n, int32_t K) {
     induce();
 }
 
-struct Ann { std::string name, anno; int64_t offset; int32_t len, n_ambs; };
-struct Amb { int64_t offset; int32_t len; char amb; };
-
-int nt4(int c) {
-    switch (c) {
-        case 'A': case 'a': return 0;
-        case 'C': case 'c': return 1;
-        case 'G': case 'g': return 2;
-        case 'T': case 't': return 3;
-        default: return 4;
-    }
-}
-
-bool write_file(const std::string &fn, const void *p, size_t n) {
-    FILE *fp = fopen(fn.c_str(), "wb");
-    if (!fp) return false;
-    bool ok = n == 0 || fwrite(p, 1, n, fp) == n;
-    return fclose(fp) == 0 && ok;
-}
-
 }  // namespace
 
 extern "C" int unc_index_build(const char *fasta_path, const char *prefix_c) {
     if (!fasta_path || !prefix_c) return UNC_E_ARG;
     const std::string prefix = prefix_c;
-    FILE *fp = fopen(fasta_path, "rb");
-    if (!fp) return UNC_E_IO;
-    // ---- parse FASTA (kseq semantics: name = first word of the header, comment = the rest)
-    std::vector<Ann> anns;
-    std::vector<Amb> ambs;
-    std::vector<uint8_t> fwd;  // one base per byte
-    srand48(11);
-    {
-        std::vector<char> buf;
-        fseek(fp, 0, SEEK_END);
-        long sz = ftell(fp);
-        fseek(fp, 0, SEEK_SET);
-        buf.resize((size_t) sz);
-        if (sz > 0 && fread(buf.data(), 1, (size_t) sz, fp) != (size_t) sz) { fclose(fp); return UNC_E_IO; }
-        fclose(fp);
-        size_t i = 0, n = buf.size();
-        while (i < n) {
-            while (i < n && buf[i] != '>') {  // skip to the next header
-                while (i < n && buf[i] != '\n') i++;
-                if (i < n) i++;
-            }
-            if (i >= n) break;
-            i++;  // '>'
-            size_t ls = i;
-            while (i < n && buf[i] != '\n') i++;
-            std::string header(buf.data() + ls, buf.data() + i);
-            if (!header.empty() && header.back() == '\r') header.pop_back();
-            if (i < n) i++;
-            Ann a;
-            size_t sp = header.find_first_of(" \t");
-            a.name = header.substr(0, sp);
-            a.anno = "(null)";
-            if (sp != std::string::npos && sp + 1 < header.size()) a.anno = header.substr(sp + 1);
-            a.offset = (int64_t) fwd.size();
-            a.n_ambs = 0;
-            int lasts = 0;
-            int64_t len = 0;
-            while (i < n && buf[i] != '>') {
-                char ch = buf[i++];
-                if (ch == '\n' || ch == '\r' || ch == ' ' || ch == '\t') continue;
-                int c = nt4(ch);
-                if (c >= 4) {
-                    if (lasts == ch) {
-                        ambs.back().len++;
-                    } else {
-                        Amb h = {a.offset + len, 1, ch};
-                        ambs.push_back(h);
-                        a.n_ambs++;
-                    }
-                    c = (int) (lrand48() & 3);
-                }
-                lasts = ch;
-                fwd.push_back((uint8_t) c);
-                len++;
-            }
-            a.len = (int32_t) len;
-            anns.push_back(a);
-        }
-    }
+    BwaRef R;
+    int rc = unc_bwa_read_fasta(fasta_path, R);
+    if (rc != UNC_OK) return rc;
+    const std::vector<uint8_t> &fwd = R.fwd;
     const int64_t l_pac = (int64_t) fwd.size();
     if (l_pac == 0) return UNC_E_IO;
     if (2 * l_pac + 1 >= 0x7FFFFFF0ll) return UNC_E_TOO_LARGE;
-
-    // ---- .pac (forward only), .ann, .amb
-    {
-        std::vector<uint8_t> pac((size_t) (l_pac >> 2) + ((l_pac & 3) == 0 ? 0 : 1), 0);
-        for (int64_t l = 0; l < l_pac; l++) pac[(size_t) (l >> 2)] |= (uint8_t) (fwd[(size_t) l] << ((~l & 3) << 1));
-        if ((l_pac % 4) == 0) pac.push_back(0);
-        pac.push_back((uint8_t) (l_pac % 4));
-        if (!write_file(prefix + ".pac", pac.data(), pac.size())) return UNC_E_IO;
-        FILE *fa = fopen((prefix + ".ann").c_str(), "w");
-        if (!fa) return UNC_E_IO;
-        fprintf(fa, "%lld %d %u\n", (long long) l_pac, (int) anns.size(), 11u);
-        for (const Ann &a : anns) {
-            fprintf(fa, "%d %s", 0, a.name.c_str());
-            if (!a.anno.empty()) fprintf(fa, " %s\n", a.anno.c_str());
-            else fprintf(fa, "\n");
-            fprintf(fa, "%lld %d %d\n", (long long) a.offset, a.len, a.n_ambs);
-        }
-        fclose(fa);
-        fa = fopen((prefix + ".amb").c_str(), "w");
-        if (!fa) return UNC_E_IO;
-        fprintf(fa, "%lld %d %u\n", (long long) l_pac, (int) anns.size(), (unsigned) ambs.size());
-        for (const Amb &h : ambs) fprintf(fa, "%lld %d %c\n", (long long) h.offset, h.len, h.amb);
-        fclose(fa);
-    }
+    if ((rc = unc_bwa_write_pac_ann_amb(R, prefix)) != UNC_OK) return rc;
 
     // ---- text = forward + reverse complement, suffix array, BWT
     const int64_t n = 2 * l_pac;  // bwt->seq_len
@@ -242,28 +146,13 @@ extern "C" int unc_index_build(const char *fasta_path, const char *prefix_c) {
         memcpy(&out[k], c, 32);
         if (k + 8 != bwt_words) return UNC_E_IO;
     }
+    if ((rc = unc_bwa_write_bwt(prefix, primary, L2, out.data(), out.size())) != UNC_OK) return rc;
+    // ---- sampled SA: rows 32, 64, ...
     {
-        FILE *fb = fopen((prefix + ".bwt").c_str(), "wb");
-        if (!fb) return UNC_E_IO;
-        fwrite(&primary, 8, 1, fb);
-        fwrite(&L2[1], 8, 4, fb);
-        fwrite(out.data(), 4, out.size(), fb);
-        if (fclose(fb) != 0) return UNC_E_IO;
-    }
-    // ---- sampled SA: rows 32, 64, ... (row 0 is written as -1 on load and not stored)
-    {
-        const uint64_t sa_intv = 32, seq_len = (uint64_t) n;
-        const uint64_t n_sa = (seq_len + sa_intv) / sa_intv;
+        const uint64_t seq_len = (uint64_t) n, n_sa = unc_bwa_n_sa(seq_len);
         std::vector<uint64_t> sa((size_t) n_sa, 0);
-        for (uint64_t j = 1; j < n_sa; j++) sa[(size_t) j] = (uint64_t) SA[(size_t) (j * sa_intv)];
-        FILE *fs = fopen((prefix + ".sa").c_str(), "wb");
-        if (!fs) return UNC_E_IO;
-        fwrite(&primary, 8, 1, fs);
-        fwrite(&L2[1], 8, 4, fs);
-        fwrite(&sa_intv, 8, 1, fs);
-        fwrite(&seq_len, 8, 1, fs);
-        fwrite(sa.data() + 1, 8, (size_t) (n_sa - 1), fs);
-        if (fclose(fs) != 0) return UNC_E_IO;
+        for (uint64_t j = 1; j < n_sa; j++) sa[(size_t) j] = (uint64_t) SA[(size_t) (j * UNC_BWA_SA_INTV)];
+        if ((rc = unc_bwa_write_sa(prefix, primary, L2, seq_len, sa.data() + 1)) != UNC_OK) return rc;
     }
     return UNC_OK;
 }

@@ -1,5 +1,6 @@
 """`uncalled index` (reference scripts/uncalled:38-78) on this package's native library: the bwa-compatible FM
-index (`BwaIndex.create`, reference src/bwa_index.hpp:92-101 -> unc_index_build), the sampled self-alignments
+index (`BwaIndex.create`, reference src/bwa_index.hpp:92-101 -> unc_index_build_device on a GPU machine,
+unc_index_build otherwise), the sampled self-alignments
 (`self_align`, reference src/self_align_ref.cpp:34-91, src/pybinder.cpp:59 -> unc_self_align on the GPU) and the
 parameter search that turns them into the `.uncl` thresholds (index_params.py).  No CPU fallback: `self_align`
 raises UncError without a usable CUDA device."""
@@ -19,8 +20,12 @@ UNCL_SUFF = ".uncl"
 class BwaIndex:
     @staticmethod
     def create(fasta_filename, bwa_prefix):
-        """BwaIndex<K>::create (src/bwa_index.hpp:92-101): <prefix>.pac/.ann/.amb/.bwt/.sa as bwa writes them."""
-        N.check(N.lib().unc_index_build(os.fsencode(fasta_filename), os.fsencode(bwa_prefix)))
+        """BwaIndex<K>::create (src/bwa_index.hpp:92-101): <prefix>.pac/.ann/.amb/.bwt/.sa as bwa writes them.  Built
+        on the GPU (unc_index_build_device) when a CUDA device is visible, by the host builder otherwise: the files are
+        the same, byte for byte."""
+        L = N.lib()
+        build = L.unc_index_build_device if L.unc_device_count() > 0 else L.unc_index_build
+        N.check(build(os.fsencode(fasta_filename), os.fsencode(bwa_prefix)))
 
 
 def self_align_csr(bwa_prefix, sample_dist):
