@@ -278,6 +278,10 @@ int unc_stream_set_tie_order(unc_stream *st, int mode);
  * wall-clock time of the last step, copies included (the per-chunk decision latency a ReadUntil client sees). */
 int unc_stream_set_chunk_timeout(unc_stream *st, float ms);
 float unc_stream_last_step_ms(const unc_stream *st);
+/* The channel's streaming normaliser (Mapper::norm_, src/normalizer.hpp:76-78) as the last step left it: mean_ and
+ * varsum_ (Normalizer::get_mean = mean, get_stdv = sqrt(varsum / n)), n_ (events in the window, at most 6000) and the
+ * ring cursor wr_.  Read-only; for inspection and tests. */
+int unc_stream_channel_norm(const unc_stream *st, uint32_t channel, double *mean, double *varsum, uint32_t *n, uint32_t *wr);
 void unc_stream_free(unc_stream *st);
 
 /* ---- `uncalled index` after the BWA build ----------------------------------------------------------

@@ -271,8 +271,11 @@ int ref_stream_read(const float *sig, uint32_t n, float chunk_time, uint32_t max
 
 // Several reads one after the other through ONE Mapper, as the reads of one channel reach a
 // RealtimePool (the Mapper's streaming normaliser and sources_added_ persist between reads).
-int ref_stream_channel(const float *samples, const uint64_t *offsets, const uint32_t *lens, uint32_t n_reads,
-                       float chunk_time, uint32_t max_chunks, ref_paf_rec *out, uint32_t *n_chunks_used, int32_t *ended) {
+// norm_state (optional, 4 per read): the Mapper's streaming Normalizer after the read, (mean_, varsum_, n_, wr_)
+// (src/normalizer.hpp:76-78), read directly from its members.
+int ref_stream_channel_norm(const float *samples, const uint64_t *offsets, const uint32_t *lens, uint32_t n_reads,
+                            float chunk_time, uint32_t max_chunks, ref_paf_rec *out, uint32_t *n_chunks_used, int32_t *ended,
+                            double *norm_state) {
     Mapper::PRMS.evt_timeout = 1e30f;
     Mapper::PRMS.chunk_timeout = 1e30f;
     float old_ct = ReadBuffer::PRMS.chunk_time;
@@ -280,11 +283,21 @@ int ref_stream_channel(const float *samples, const uint64_t *offsets, const uint
     ReadBuffer::PRMS.chunk_time = chunk_time;
     ReadBuffer::PRMS.max_chunks = max_chunks;
     Mapper m;
-    for (uint32_t i = 0; i < n_reads; i++)
+    for (uint32_t i = 0; i < n_reads; i++) {
         stream_one(m, samples + offsets[i], lens[i], i + 1, out + i, n_chunks_used ? n_chunks_used + i : nullptr,
                    ended ? ended + i : nullptr);
+        if (norm_state) {
+            double *s = norm_state + (size_t) 4 * i;
+            s[0] = m.norm_.mean_; s[1] = m.norm_.varsum_; s[2] = m.norm_.n_; s[3] = m.norm_.wr_;
+        }
+    }
     ReadBuffer::PRMS.chunk_time = old_ct; ReadBuffer::PRMS.max_chunks = old_mc;
     return 0;
+}
+
+int ref_stream_channel(const float *samples, const uint64_t *offsets, const uint32_t *lens, uint32_t n_reads,
+                       float chunk_time, uint32_t max_chunks, ref_paf_rec *out, uint32_t *n_chunks_used, int32_t *ended) {
+    return ref_stream_channel_norm(samples, offsets, lens, n_reads, chunk_time, max_chunks, out, n_chunks_used, ended, nullptr);
 }
 
 // A flow cell's worth of channels on n_threads worker threads: read i sits on channel i % n_channels, the reads of a

@@ -1532,6 +1532,7 @@ typedef struct {
     snorm_t norm;
     evprof_t prof;
     evdt_t ed;
+    u64 n_pushed;           /* successful normaliser pushes so far (reporting only) */
 } stream_chan_t;
 
 static void chan_init(stream_chan_t *c, const orc_index *idx, const orc_model *m, const orc_params *p) {
@@ -1540,6 +1541,7 @@ static void chan_init(stream_chan_t *c, const orc_index *idx, const orc_model *m
     snorm_init(&c->prof.window, EVP_WIN, 0, 0);
     evprof_reset(&c->prof);
     evdt_reset(&c->ed, p);
+    c->n_pushed = 0;
 }
 static void chan_free(stream_chan_t *c) {
     free(c->norm.signal); free(c->prof.window.signal);
@@ -1596,6 +1598,7 @@ static void chan_map_read(stream_chan_t *c, const float *raw, uint32_t n, uint32
                     if (!snorm_push(norm, evt_mean)) goto chunk_done;   /* returns with the chunk unprocessed */
                 }
                 nevents++;
+                c->n_pushed++;
             }
             chunk_processed = 1;
         }
@@ -1648,16 +1651,54 @@ int orc_stream_map_read(const orc_index *idx, const orc_model *m, const orc_para
     return 0;
 }
 
+/* orc_stream_map_channel, and after every read the channel's streaming normaliser:
+ * norm_state (optional, 4 per read): its (mean_, varsum_, n_, wr_) after the read;
+ * n_pushed (optional, 1 per read): the channel's normaliser pushes so far. */
+int orc_stream_map_channel_norm(const orc_index *idx, const orc_model *m, const orc_params *p, const float *samples,
+                                const uint64_t *offsets, const uint32_t *lens, uint32_t n_reads, uint32_t chunk_len,
+                                uint32_t max_chunks, orc_paf_rec *out, uint32_t *n_chunks_used, int32_t *ended,
+                                double *norm_state, uint64_t *n_pushed) {
+    stream_chan_t c;
+    chan_init(&c, idx, m, p);
+    for (uint32_t i = 0; i < n_reads; i++) {
+        chan_map_read(&c, samples + offsets[i], lens[i], chunk_len, max_chunks, out + i,
+                      n_chunks_used ? n_chunks_used + i : NULL, ended ? ended + i : NULL);
+        if (norm_state) {
+            double *s = norm_state + (size_t) 4 * i;
+            s[0] = c.norm.mean; s[1] = c.norm.varsum; s[2] = c.norm.n; s[3] = c.norm.wr;
+        }
+        if (n_pushed) n_pushed[i] = c.n_pushed;
+    }
+    chan_free(&c);
+    return 0;
+}
+
 /* Several reads one after the other on ONE channel (the channel's Mapper persists, as in RealtimePool). */
 int orc_stream_map_channel(const orc_index *idx, const orc_model *m, const orc_params *p, const float *samples,
                            const uint64_t *offsets, const uint32_t *lens, uint32_t n_reads, uint32_t chunk_len,
                            uint32_t max_chunks, orc_paf_rec *out, uint32_t *n_chunks_used, int32_t *ended) {
-    stream_chan_t c;
-    chan_init(&c, idx, m, p);
-    for (uint32_t i = 0; i < n_reads; i++)
-        chan_map_read(&c, samples + offsets[i], lens[i], chunk_len, max_chunks, out + i,
-                      n_chunks_used ? n_chunks_used + i : NULL, ended ? ended + i : NULL);
-    chan_free(&c);
+    return orc_stream_map_channel_norm(idx, m, p, samples, offsets, lens, n_reads, chunk_len, max_chunks, out,
+                                       n_chunks_used, ended, NULL, NULL);
+}
+
+/* The events process_chunk pushes into the normaliser, without the mapper: the detector and the event profiler over
+ * n_chunks chunks of one read (both start afresh, as at Mapper::new_read).  cum_pushed[k]: pushes after chunk k. */
+int orc_stream_chunk_pushes(const orc_params *p, const float *raw, uint32_t n_chunks, uint32_t chunk_len,
+                            uint32_t *cum_pushed) {
+    evdt_t ed;
+    evprof_t prof;
+    evdt_reset(&ed, p);
+    snorm_init(&prof.window, EVP_WIN, 0, 0);
+    evprof_reset(&prof);
+    u32 n = 0;
+    for (u32 k = 0; k < n_chunks; k++) {
+        for (u32 i = 0; i < chunk_len; i++) {
+            if (!evdt_add_sample(&ed, raw[(size_t) k * chunk_len + i])) continue;
+            if (evprof_add(&prof, ed.ev_mean)) n++;
+        }
+        cum_pushed[k] = n;
+    }
+    free(prof.window.signal);
     return 0;
 }
 

@@ -303,6 +303,7 @@ struct EmuStream {
     std::vector<u32> order;
     DevWork W;
     DevWorkStrides S;
+    std::vector<std::vector<float>> pushed;   // per channel: every event mean unc_stream_chunk emitted, in order
 };
 struct StreamCtaArgs { const DevIndex *ix; const DevParams *p; const DevBatch *B; const DevWork *W; const DevWorkStrides *S; K2Shared *sh; };
 static void stream_cta_entry(void *a) {
@@ -318,6 +319,7 @@ void *emu_stream_create(void *pidx, const unc_params *prm, uint32_t n_channels, 
     T->n_channels = n_channels; T->max_chunk_len = max_chunk_len; T->max_chunks = max_chunks;
     T->ev_stride = (max_chunk_len + 3u) & ~3u; T->max_blocks = max_blocks;
     T->ch.resize(n_channels);
+    T->pushed.resize(n_channels);
     T->sig.resize(n_channels); memset(T->sig.data(), 0, n_channels * sizeof(DevChanSig));
     T->norm_sig.assign((size_t) n_channels * UNC_NORM_LEN, 0.0f);
     T->map.resize(n_channels); memset(T->map.data(), 0, n_channels * sizeof(DevMapState));
@@ -382,6 +384,8 @@ int emu_stream_step(void *pst, const unc_chunk_desc *chunks, uint32_t n, const v
         for (u32 r = 0; r < m; r++) {
             unc_stream_chunk(B, T->dp, S, r, isnew[r]);
             tot[r] = T->sig[chan[r]].evdt.total_events;
+            const float *ev = events.data() + (size_t) r * T->ev_stride;
+            T->pushed[chan[r]].insert(T->pushed[chan[r]].end(), ev, ev + n_events[r]);
         }
         K2Shared *sh = (K2Shared *) calloc(1, K2_SMEM_BYTES(T->dp.max_paths));
         StreamCtaArgs a = {&T->e->ix, &T->dp, &B, &T->W, &T->S, sh};
@@ -398,6 +402,19 @@ int emu_stream_step(void *pst, const unc_chunk_desc *chunks, uint32_t n, const v
         stream_result(h, bp_per_samp, &out[i]);
     }
     return 0;
+}
+
+// The channel's streaming normaliser as the device left it: state = (mean, varsum, n, wr) of DevChanSig.norm, ring (optional,
+// UNC_NORM_LEN floats) = its slice of DevStream::norm_sig.  Returns the number of event means the channel has pushed so far;
+// pushed (optional, cap floats) receives the first min(cap, that number) of them.
+uint64_t emu_stream_norm_state(void *pst, uint32_t channel, double *state, float *ring, float *pushed, uint64_t cap) {
+    EmuStream *T = (EmuStream *) pst;
+    const DevRing &z = T->sig[channel].norm;
+    state[0] = z.mean; state[1] = z.varsum; state[2] = z.n; state[3] = z.wr;
+    if (ring) memcpy(ring, T->norm_sig.data() + (size_t) channel * UNC_NORM_LEN, UNC_NORM_LEN * sizeof(float));
+    const std::vector<float> &p = T->pushed[channel];
+    if (pushed) memcpy(pushed, p.data(), std::min<uint64_t>(cap, p.size()) * sizeof(float));
+    return p.size();
 }
 
 // ---- self_align: the device functions of unc_selfalign.cuh, one "thread" after the other, around the same

@@ -105,6 +105,8 @@ def _bind(L):
     L.emu_stream_create.argtypes = [C.c_void_p, C.POINTER(UncParams), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
     L.emu_stream_free.argtypes = [C.c_void_p]
     L.emu_stream_step.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_int]
+    L.emu_stream_norm_state.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
+    L.emu_stream_norm_state.restype = C.c_uint64
     return L
 
 
@@ -186,6 +188,21 @@ class EmuStream:
 
     def map_reads(self, signals, chunk_len):
         return stream_reads(self.step, self.n_channels, signals, chunk_len, self.max_chunks)
+
+    def norm_state(self, channel, ring=False, pushed=False):
+        """The channel's streaming normaliser: (mean, varsum, n, wr) as float64, then with ring=True its 6000-float ring,
+        with pushed=True every event mean the channel has pushed so far."""
+        st = np.zeros(4, np.float64)
+        rg = np.zeros(6000, np.float32) if ring else None
+        n = self.emu.L.emu_stream_norm_state(self.h, channel, st.ctypes.data, None if rg is None else rg.ctypes.data, None, 0)
+        out = [st]
+        if ring:
+            out.append(rg)
+        if pushed:
+            pv = np.zeros(max(int(n), 1), np.float32)
+            self.emu.L.emu_stream_norm_state(self.h, channel, st.ctypes.data, None, pv.ctypes.data, n)
+            out.append(pv[:n])
+        return out[0] if len(out) == 1 else tuple(out)
 
     def close(self):
         if self.h:

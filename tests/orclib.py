@@ -7,6 +7,7 @@ cpu_baseline / --impl reference legs, never by the product package.
 import ctypes as C
 import os
 import subprocess
+import sys
 import tempfile
 
 import numpy as np
@@ -117,6 +118,8 @@ def orc():
         lib.orc_stream_map_channel.argtypes = [C.c_void_p, C.POINTER(OrcModel), C.POINTER(OrcParams), f32p, u64p, u32p,
                                                C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(OrcPaf),
                                                C.POINTER(C.c_uint32), C.POINTER(C.c_int32)]
+        lib.orc_stream_map_channel_norm.argtypes = lib.orc_stream_map_channel.argtypes + [C.c_void_p, C.c_void_p]
+        lib.orc_stream_chunk_pushes.argtypes = [C.POINTER(OrcParams), f32p, C.c_uint32, C.c_uint32, u32p]
         _orc = lib
     return _orc
 
@@ -179,15 +182,29 @@ class Oracle:
 
     def stream_channel(self, signals, chunk_len, max_chunks=1000000):
         """Reads one after the other on one channel (persistent Mapper); returns [(rec, chunks, ended)]."""
+        return self.stream_channel_norm(signals, chunk_len, max_chunks)[0]
+
+    def stream_channel_norm(self, signals, chunk_len, max_chunks=1000000):
+        """stream_channel, and after every read the channel's streaming normaliser: (results, state, pushed) with
+        state[i] = (mean_, varsum_, n_, wr_) as float64 and pushed[i] = the normaliser pushes so far (uint64)."""
         flat = np.ascontiguousarray(np.concatenate(signals), dtype=np.float32)
         lens = np.array([len(s) for s in signals], np.uint32)
         offs = np.concatenate([[0], np.cumsum(lens[:-1], dtype=np.uint64)]).astype(np.uint64)
         n = len(signals)
         out, nu, en = (OrcPaf * n)(), (C.c_uint32 * n)(), (C.c_int32 * n)()
-        self.lib.orc_stream_map_channel(self.idx, C.byref(self.model), C.byref(self.params), fp(flat),
-                                        offs.ctypes.data_as(u64p), lens.ctypes.data_as(u32p), n, int(chunk_len),
-                                        int(max_chunks), out, nu, en)
-        return [(out[i], nu[i], en[i]) for i in range(n)]
+        state, pushed = np.zeros((n, 4), np.float64), np.zeros(n, np.uint64)
+        self.lib.orc_stream_map_channel_norm(self.idx, C.byref(self.model), C.byref(self.params), fp(flat),
+                                             offs.ctypes.data_as(u64p), lens.ctypes.data_as(u32p), n, int(chunk_len),
+                                             int(max_chunks), out, nu, en, state.ctypes.data, pushed.ctypes.data)
+        return [(out[i], nu[i], en[i]) for i in range(n)], state, pushed
+
+    def chunk_pushes(self, raw, chunk_len, n_chunks=None):
+        """Normaliser pushes after each full chunk of one read (event detector + profiler only, no mapping)."""
+        raw = np.ascontiguousarray(raw, dtype=np.float32)
+        k = raw.size // chunk_len if n_chunks is None else int(n_chunks)
+        out = np.zeros(max(k, 1), np.uint32)
+        self.lib.orc_stream_chunk_pushes(C.byref(self.params), fp(raw), k, int(chunk_len), out.ctypes.data_as(u32p))
+        return out[:k]
 
     def map_batch(self, samples, offsets, lens, threads=1):
         samples = np.ascontiguousarray(samples, dtype=np.float32)
@@ -233,11 +250,35 @@ class Oracle:
         return st, en
 
 
+_job_oracles = {}
+
+
+def stream_channel_job(args):
+    """(prefix, reads, chunk_len, child_sort): one channel through Oracle.stream_channel_norm, as a process-pool job.
+    child_sort 1 = the reference's pdqsort child sort (orc_set_child_sort).  Returns ([(PAF fields, chunks, ended,
+    (n_children, n_sources, n_seeds))], state, pushed)."""
+    prefix, reads, chunk_len, child_sort = args
+    if prefix not in _job_oracles:
+        _job_oracles[prefix] = Oracle(prefix)
+    O = _job_oracles[prefix]
+    O.lib.orc_set_child_sort(int(child_sort))
+    res, state, pushed = O.stream_channel_norm(reads, chunk_len)
+    return [(paf_tuple(r), int(nu), int(en), (int(r.n_children), int(r.n_sources), int(r.n_seeds)))
+            for r, nu, en in res], state, pushed
+
+
 _ref = None
 
 
-def ref_available():
-    return os.path.exists(os.path.join(ORACLE_DIR, "_ref", "libuncalled_ref.so"))
+def ref_available(symbol=None):
+    """oracle/_ref is built (and, with `symbol`, exports it: a prebuilt library may predate a shim function)."""
+    path = os.path.join(ORACLE_DIR, "_ref", "libuncalled_ref.so")
+    if not os.path.exists(path):
+        return False
+    if symbol is None:
+        return True
+    code = "import ctypes, sys; sys.exit(0 if hasattr(ctypes.CDLL(%r), %r) else 1)" % (path, symbol)
+    return subprocess.run([sys.executable, "-c", code], capture_output=True).returncode == 0
 
 
 def ref(stable_sort=False):
@@ -270,6 +311,9 @@ def ref(stable_sort=False):
         lib.ref_map_batch_mt.argtypes = [f32p, u64p, u32p, C.c_uint32, C.c_int, C.POINTER(RefPaf)]
         lib.ref_stream_channel.argtypes = [f32p, u64p, u32p, C.c_uint32, C.c_float, C.c_uint32, C.POINTER(RefPaf),
                                            C.POINTER(C.c_uint32), C.POINTER(C.c_int32)]
+        if hasattr(lib, "ref_stream_channel_norm"):     # absent from an oracle/_ref built before it was added
+            lib.ref_stream_channel_norm.argtypes = [f32p, u64p, u32p, C.c_uint32, C.c_float, C.c_uint32, C.POINTER(RefPaf),
+                                                    C.POINTER(C.c_uint32), C.POINTER(C.c_int32), C.c_void_p]
         lib.ref_stream_channels_mt.argtypes = [f32p, u64p, u32p, C.c_uint32, C.c_uint32, C.c_float, C.c_uint32, C.c_int,
                                                C.POINTER(RefPaf), C.POINTER(C.c_uint32), C.POINTER(C.c_int32)]
         lib.ref_stream_read.argtypes = [f32p, C.c_uint32, C.c_float, C.c_uint32, C.POINTER(RefPaf),

@@ -82,7 +82,7 @@ EXPORTS = ["unc_strerror", "unc_last_error", "unc_device_count", "unc_init", "un
            "unc_index_load", "unc_index_get_info", "unc_index_seq", "unc_index_kmer_range",
            "unc_index_thresholds", "unc_index_free", "unc_index_build", "unc_pool_create", "unc_pool_free",
            "unc_map_batch", "unc_map_batch_device", "unc_map_batch_ordered", "unc_pool_set_tie_order", "unc_map_batch_submit", "unc_map_batch_wait", "unc_pool_record", "unc_pool_elapsed", "unc_events_batch", "unc_match_probs", "unc_fm_neighbors",
-           "unc_fm_sa", "unc_pool_last_timing", "unc_pool_k1_stats", "unc_stream_create", "unc_stream_set_tie_order", "unc_stream_set_chunk_timeout", "unc_stream_last_step_ms", "unc_stream_step",
+           "unc_fm_sa", "unc_pool_last_timing", "unc_pool_k1_stats", "unc_stream_create", "unc_stream_set_tie_order", "unc_stream_set_chunk_timeout", "unc_stream_last_step_ms", "unc_stream_channel_norm", "unc_stream_step",
            "unc_stream_free", "unc_self_align", "unc_free", "unc_fast5_open", "unc_fast5_count", "unc_fast5_info",
            "unc_fast5_load", "unc_fast5_close", "unc_fast5_last_error", "unc_dtw_batch", "unc_dtw_release", "unc_dtw_last_kernel_ms",
            "unc_mask_internal", "unc_mask_last_kernel_ms", "unc_mask_external", "unc_mask_external_last_kernel_ms",
@@ -185,6 +185,7 @@ def lib():
     L.unc_stream_set_chunk_timeout.argtypes = [vp, C.c_float]
     L.unc_stream_last_step_ms.argtypes = [vp]
     L.unc_stream_last_step_ms.restype = C.c_float
+    L.unc_stream_channel_norm.argtypes = [vp, u32, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(u32), C.POINTER(u32)]
     L.unc_stream_free.argtypes = [vp]
     L.unc_stream_free.restype = None
     L.unc_self_align.argtypes = [C.c_char_p, u32, C.POINTER(C.c_uint64), C.POINTER(vp), C.POINTER(vp)]

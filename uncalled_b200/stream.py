@@ -100,6 +100,13 @@ class StreamMapper:
         """Wall-clock time of the last step (copies included): the decision latency of its chunks."""
         return float(self.L.unc_stream_last_step_ms(self.h))
 
+    def norm_state(self, channel):
+        """The channel's streaming normaliser after the last step: (mean, varsum, n, wr), n being the events in its
+        window (at most 6000) and wr its ring cursor."""
+        m, v, n, w = C.c_double(), C.c_double(), C.c_uint32(), C.c_uint32()
+        N.check(self.L.unc_stream_channel_norm(self.h, int(channel), C.byref(m), C.byref(v), C.byref(n), C.byref(w)))
+        return m.value, v.value, n.value, w.value
+
     def step(self, descs, n, flat, res):
         flat = np.ascontiguousarray(flat)
         rc = self.L.unc_stream_step(self.h, descs, n, flat.ctypes.data, res)
