@@ -318,6 +318,52 @@ int unc_dtw_batch(const float *model_means_stdvs, int cost_kind, const unc_dtw_p
 void unc_dtw_release(void);
 float unc_dtw_last_kernel_ms(void);
 
+/* ---- signal-level alignment of reads to reference spans (the reference's dtw_test driver) ---------------------
+ *   unc_dtw_aligner_create  BwaIndex<KLEN> idx(prefix); idx.load_pacseq(); pmodel_r94_template
+ *                                                      src/dtw_test.cpp:74-81 (host only: the device copy of the .pac is
+ *                                                      made by the first batch)
+ *   unc_dtw_aligner_contig  BwaIndex::coord_to_pacseq's contig lookup by name    src/bwa_index.hpp:226-233
+ *   unc_dtw_align_batch     the loop body of dtw_test per query, for many reads at once   src/dtw_test.cpp:94-175:
+ *                           EventDetector::get_events over the signal (no max_events cap), EventProfiler::get_full_mask
+ *                           and the unmasked means, BwaIndex::get_kmers(rf_name, rf_st, rf_en) (+ kmers_revcomp unless
+ *                           fwd), Normalizer(read_mean, read_stdv) from the span's template model means, the > 50 000
+ *                           means skip, DTWr94d(means, kmers, {NONE, 1, 1, 1}) and mean_score()
+ *   unc_dtw_align_path      DTW::get_path() of one aligned query of the last batch   src/dtw.hpp:124-126
+ * reads[i] is the signal of query i: samples [rd_st, rd_en) of the read, as unc_map_batch takes them (one dtype per batch).
+ * Every query gets a status: UNC_DTW_ALIGN_OK, or the reason it was skipped (the other queries are unaffected).  The
+ * sweep runs in launches whose breadcrumb matrices (one byte per cell) and work arrays fit the budget (default: the free
+ * device memory less 128 MiB); a query whose matrix alone exceeds it is skipped with UNC_DTW_ALIGN_TOO_LARGE.  Queries
+ * skipped by the host checks (unknown contig, span past the contig's end or shorter than 5 bases, empty signal) never
+ * reach the device: a batch made only of them does not touch it.  With keep_paths, unc_dtw_align_path copies query i's
+ * path, path_len (column = event index, row = k-mer index) u64 pairs from the end cell back to the start, as
+ * unc_dtw_batch returns them, and (each optional) its n_kept normalised means and its n_kmers = rf_en - rf_st - 4 k-mers.  unc_dtw_align_last_times: CUDA-event times of the last batch in ms (H2D, stages (a)-(e)
+ * of unc_dtw_align.cuh, the sweep launches, total), the number of sweep launches and of matrix cells. */
+#define UNC_DTW_ALIGN_OK 0
+#define UNC_DTW_ALIGN_TOO_MANY_MEANS 1   /* more than 50 000 means after the mask (dtw_test.cpp:156-159) */
+#define UNC_DTW_ALIGN_NO_EVENTS 2        /* no event left after the mask */
+#define UNC_DTW_ALIGN_TOO_LARGE 3        /* the matrix alone exceeds the workspace budget */
+#define UNC_DTW_ALIGN_UNKNOWN_CONTIG 4
+#define UNC_DTW_ALIGN_SPAN_PAST_END 5    /* rf_en past the contig's end (or rf_st > rf_en) */
+#define UNC_DTW_ALIGN_SPAN_SHORT 6       /* fewer than 5 bases: no k-mer */
+#define UNC_DTW_ALIGN_EMPTY_SIGNAL 7
+typedef struct unc_dtw_aligner unc_dtw_aligner;
+typedef struct { int32_t rid; uint32_t fwd; uint64_t rf_st, rf_en; } unc_dtw_query;
+typedef struct {
+    int32_t status;
+    uint32_t n_events, n_kept;       /* events detected; means left after the mask */
+    float score, mean_score;
+    uint32_t pad;
+    uint64_t path_len;
+} unc_dtw_align_result;
+int unc_dtw_aligner_create(const char *bwa_prefix, const char *model_table_path, unc_dtw_aligner **out);
+void unc_dtw_aligner_free(unc_dtw_aligner *a);
+int unc_dtw_aligner_contig(const unc_dtw_aligner *a, const char *name, int32_t *rid, uint64_t *len);
+int unc_dtw_aligner_set_budget(unc_dtw_aligner *a, uint64_t bytes);
+int unc_dtw_align_batch(unc_dtw_aligner *a, uint32_t n, const unc_read_desc *reads, const void *samples,
+                        const unc_dtw_query *q, int keep_paths, unc_dtw_align_result *res);
+int unc_dtw_align_path(const unc_dtw_aligner *a, uint32_t i, uint64_t *pairs, float *means, uint16_t *kmers);
+int unc_dtw_align_last_times(const unc_dtw_aligner *a, float ms[8], uint64_t *launches, uint64_t *cells);
+
 /* ---- iterative high-frequency k-mer masking of a reference (`mask-internal`) -----------------------------------
  *   unc_mask_internal   masking/mask_internal.sh <reference> <k> <iters> <out_prefix>: per iteration `jellyfish count`
  *                       (forward strand, no -C), the k-mer of the maximum count, masking/mask_kmers.py -k <kmer>

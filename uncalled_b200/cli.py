@@ -100,6 +100,18 @@ def get_parser(conf):
                    "<out_prefix>reps_m<min_copy>.bed")
     p.add_argument("--device", type=int, default=0, help="CUDA device")
 
+    p = sp.add_parser("dtw", help="Align reads to known reference spans at the signal level (DTW of the read's "
+                      "normalised event means against the span's k-mers)", formatter_class=fmt)
+    p.add_argument("bwa_prefix", type=str, help="BWA prefix of the reference (only the .pac and .ann are read)")
+    p.add_argument("fast5s", nargs="+", type=str, help="Reads to align. Can be a directory which will be recursively "
+                   "searched for all files with the \".fast5\" extension, a text file containing one fast5 filename per "
+                   "line, or a comma-separated list of fast5 file names.")
+    p.add_argument("--queries", required=True, type=str, help="One query per line: rd_name rd_st rd_en rf_name rf_st "
+                   "rf_en strand (samples [rd_st, rd_en) of the read, 0 0 = all of it; bases [rf_st, rf_en) of the contig)")
+    p.add_argument("--path-prefix", type=str, default="", help="Also write each read's DTW path to <prefix><read_id>.txt")
+    p.add_argument("-r", "--recursive", action="store_true", help="Recursively search 'fast5s' for fast5 files")
+    p.add_argument("--device", type=int, default=0, help="CUDA device")
+
     p = sp.add_parser("pafstats",help="Computes speed and accuracy of UNCALLED mappings.", formatter_class=fmt)
     p.add_argument("infile", type=str, help="PAF file output by UNCALLED")          # uncalled/pafstats.py:165-169
     p.add_argument("-n", "--max-reads", required=False, type=int, default=None, help="Will only look at first n reads if specified")
@@ -202,6 +214,69 @@ def sim_cmd(conf, args, out=None):
     sys.stderr.write("Finished\n")
 
 
+def dtw_cmd(args, out=None):
+    """src/dtw_test.cpp: the reads named in the query file, in the order the fast5 files hand them out, aligned on the GPU.
+    stdout: read_id, mean score, seconds.  A bad query file ends the command with status 1 before the GPU is touched."""
+    from concurrent.futures import ThreadPoolExecutor
+    from . import _native as N
+    from .dtw import DtwAligner, QueryError, format_path, host_skip, load_queries
+    from .fast5 import Fast5File
+    out = out or sys.stdout
+    for ext in (".pac", ".ann"):
+        assert_exists(args.bwa_prefix + ext)
+    assert_exists(args.queries)
+    aligner = DtwAligner(args.bwa_prefix)
+    try:
+        queries = load_queries(args.queries, aligner)
+    except QueryError as e:
+        sys.stderr.write("Error: %s\n" % e)
+        sys.exit(1)
+    files = [f for f in load_fast5s(args.fast5s, args.recursive) if f is not None]
+
+    def batches(max_reads=64, max_samples=1 << 25):
+        """the queried reads, decoded file by file (Fast5Reader::add_read filter), in batches of one signal type"""
+        batch, n = [], 0
+        for path in files:
+            with Fast5File(path) as f:
+                for i in range(f.n_reads):
+                    if f.info(i).read_id not in queries:
+                        continue
+                    r = f.load(i, 1)[0]
+                    if batch and (len(batch) >= max_reads or n + len(r.signal) > max_samples):
+                        yield batch
+                        batch, n = [], 0
+                    batch.append(r)
+                    n += len(r.signal)
+        if batch:
+            yield batch
+
+    gpu_ready = False
+    with ThreadPoolExecutor(max_workers=1) as ex:     # the next batch is decoded while the GPU aligns this one
+        it = batches()
+        fut = ex.submit(next, it, None)
+        while True:
+            batch = fut.result()
+            if batch is None:
+                break
+            fut = ex.submit(next, it, None)
+            t0 = time.time()
+            qs = [(r.read_id, r.signal, r.calibration) + queries[r.read_id] for r in batch]
+            if not gpu_ready and any(host_skip(aligner, len(q[1]), *q[3:8]) is None for q in qs):
+                N.check(N.lib().unc_init(args.device))
+                gpu_ready = True
+            res = aligner.align(qs, paths=bool(args.path_prefix))
+            secs = (time.time() - t0) / len(res)
+            for a in res:
+                if a.skip is not None:
+                    sys.stderr.write(a.skip_message() + "\n")
+                    continue
+                if args.path_prefix:
+                    with open(args.path_prefix + a.read_id + ".txt", "w") as pf:
+                        pf.write(format_path(a))
+                out.write("%s\t%g\t%g\n" % (a.read_id, a.mean_score, secs))
+            out.flush()
+
+
 def load_conf(argv):
     """uncalled/args.py:288-302: every parsed option whose name is a Conf attribute is set on the Conf."""
     from .api import Conf
@@ -238,6 +313,8 @@ def main(argv=None):
         N.check(N.lib().unc_init(args.device))
         masked, _ = mask_external(args.full_reference, args.target, args.min_len, args.min_copy, args.out_prefix)
         sys.stdout.write("Masked %d basepairs\n" % masked)
+    elif args.subcmd == "dtw":
+        dtw_cmd(args)
     elif args.subcmd == "pafstats":
         from . import pafstats
         pafstats.run(args.infile, args.ref_paf, args.max_reads)

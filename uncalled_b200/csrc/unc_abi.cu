@@ -885,6 +885,7 @@ int unc_pool_last_timing(const unc_pool *P, unc_timing *t) {
 #include "unc_stream_host.inl"
 #include "unc_selfalign_host.inl"
 #include "unc_dtw_host.inl"
+#include "unc_dtw_align_host.inl"
 #include "unc_mask_host.inl"
 #include "unc_mask_ext_host.inl"
 #include "unc_fmb_host.inl"

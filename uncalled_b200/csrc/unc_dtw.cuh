@@ -32,7 +32,7 @@ struct DevDtw {
     float *diag, *edge;
     u64 *path, *path_len;
     float *score;
-    int cost_kind, subseq;    // 0 DTWr94p / 1 DTWr94d; DTWSubSeq 0 NONE, 1 ROW, 2 COL
+    int cost_kind, subseq;    // 0 DTWr94p / 1 DTWr94d / 2 DTWr94d with float abs (the dtw_test driver); DTWSubSeq 0 NONE, 1 ROW, 2 COL
     float dw, hw, vw;
     u32 *queue;
 };
@@ -43,6 +43,7 @@ struct DevDtw {
 
 UNC_DEV float unc_dtw_cost(const DevDtw &D, u32 kmer, float e) {
     if (D.cost_kind == 0) return -unc_match_prob(e, D.model[kmer], D.model[1024 + kmer], D.model[2048 + kmer]);
+    if (D.cost_kind == 2) return fabsf(f_sub(e, D.model[kmer]));   // DTWr94d as dtw_test.cpp compiles it: float abs
     const int t = (int) f_sub(e, D.model[kmer]);          // int abs(int): truncation towards zero first
     return (float) (t < 0 ? -t : t);
 }

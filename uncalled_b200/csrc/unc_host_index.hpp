@@ -73,6 +73,8 @@ static inline bool hix_load_model(HostIndex &h, const std::string &table_path) {
     return true;
 }
 
+static inline bool hix_load_ann(HostIndex &h, const std::string &prefix);
+
 // The FM index proper (.bwt, .sa, .ann) -- all `uncalled index` has before the thresholds exist
 static inline bool hix_load_fm(HostIndex &h, const std::string &prefix) {
     std::vector<char> b;
@@ -104,6 +106,11 @@ static inline bool hix_load_fm(HostIndex &h, const std::string &prefix) {
         h.sa32[i] = (uint32_t) v;
     }
 
+    return hix_load_ann(h, prefix);
+}
+
+// The contigs of the .ann: names, .pac offsets and lengths (bns_restore, reference submods/bwa/bntseq.c)
+static inline bool hix_load_ann(HostIndex &h, const std::string &prefix) {
     FILE *fp = fopen((prefix + ".ann").c_str(), "r");
     if (!fp) { h.error = "cannot read " + prefix + ".ann"; return false; }
     long long xx;

@@ -5,6 +5,7 @@
 
 `dtw_batch` aligns many (means, kmers) pairs in one call (one CTA per problem on the GPU).  There is no CPU path."""
 import ctypes as C
+import os
 
 import numpy as np
 
@@ -97,3 +98,191 @@ class DTWr94d(_DTW):
     """cost = abs(event - model mean of the k-mer), as the reference compiles it: the difference is truncated to an
     integer first (src/dtw.hpp:212-232)"""
     _cost = "r94d"
+
+
+# ---------------------------------------------------------------- reads against reference spans (the dtw_test driver)
+
+class DtwQuery(C.Structure):
+    """unc_dtw_query (include/unc_b200.h)"""
+    _fields_ = [("rid", C.c_int32), ("fwd", C.c_uint32), ("rf_st", C.c_uint64), ("rf_en", C.c_uint64)]
+
+
+class DtwAlignResult(C.Structure):
+    """unc_dtw_align_result (include/unc_b200.h)"""
+    _fields_ = [("status", C.c_int32), ("n_events", C.c_uint32), ("n_kept", C.c_uint32), ("score", C.c_float),
+                ("mean_score", C.c_float), ("pad", C.c_uint32), ("path_len", C.c_uint64)]
+
+
+MAX_MEANS = 50000                     # src/dtw_test.cpp:156
+# why a query is skipped (UNC_DTW_ALIGN_* of include/unc_b200.h)
+SKIP_REASONS = {1: "too many means", 2: "no event left after the mask", 3: "the DTW matrix exceeds the workspace budget",
+                4: "unknown contig", 5: "rf_en past the end of the contig", 6: "reference span shorter than 5 bases",
+                7: "empty sample range"}
+RD_EN_PAST_END = "rd_en past the end of the signal"
+
+
+class Alignment:
+    """One query's outcome: `skip` is None when it was aligned, else the reason ("too many means" for the reference's
+    own skip above 50 000 means).  With paths: `path` = (event index, k-mer index) pairs from the start cell to the end
+    cell, `means` = the normalised kept means, `kmers` = the span's k-mers."""
+    __slots__ = ("read_id", "skip", "n_events", "n_kept", "score", "mean_score", "path", "means", "kmers")
+
+    def __init__(self, read_id, skip=None, **kw):
+        self.read_id, self.skip = read_id, skip
+        for k in self.__slots__[2:]:
+            setattr(self, k, kw.get(k))
+
+    def skip_message(self):
+        """The stderr line of a skipped query (src/dtw_test.cpp:157 for the > 50 000 means case)."""
+        return "Skipping %s" % self.read_id if self.skip == "too many means" else "Skipping %s: %s" % (self.read_id, self.skip)
+
+
+class DtwAligner:
+    """The reference's dtw_test driver (src/dtw_test.cpp:94-175) on the GPU: reads aligned by DTWr94d to their reference
+    spans, after event detection, the EventProfiler mask and normalisation to the span's model levels.  Only the .pac and
+    .ann of `bwa_prefix` are read.  `budget`: bytes of the DTW sweep's workspace (0 = the free device memory)."""
+
+    def __init__(self, bwa_prefix, budget=0):
+        self._L = N.lib()
+        self._h = C.c_void_p()
+        N.check(self._L.unc_dtw_aligner_create(os.fsencode(bwa_prefix), os.fsencode(N.MODEL_TABLE), C.byref(self._h)))
+        self.set_budget(budget)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.unc_dtw_aligner_free(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def set_budget(self, nbytes):
+        N.check(self._L.unc_dtw_aligner_set_budget(self._h, int(nbytes)))
+
+    def contig(self, name):
+        """(rid, length) of a contig of the .ann, or None"""
+        rid, ln = C.c_int32(), C.c_uint64()
+        N.check(self._L.unc_dtw_aligner_contig(self._h, name.encode(), C.byref(rid), C.byref(ln)))
+        return None if rid.value < 0 else (rid.value, ln.value)
+
+    def align(self, queries, paths=False):
+        """queries: (read_id, signal, calibration, rd_st, rd_en, contig, rf_st, rf_en, fwd) per read, all with the same
+        signal type: float32 pA (calibration None) or int16 DAC values with their (range, offset, digitisation).
+        rd_st = rd_en = 0 takes the whole signal; rd_en = 0 runs to its end.  Returns one Alignment per query, in order."""
+        n = len(queries)
+        out = [None] * n
+        descs = (N.ReadDesc * max(n, 1))()
+        qs = (DtwQuery * max(n, 1))()
+        parts, off = [], 0
+        for i, (rid_, sig, cal, rd_st, rd_en, contig, rf_st, rf_en, fwd) in enumerate(queries):
+            en = len(sig) if rd_en == 0 else rd_en
+            c = self.contig(contig)
+            qs[i].rid, qs[i].fwd, qs[i].rf_st, qs[i].rf_en = (c[0] if c else -1), int(bool(fwd)), int(rf_st), int(rf_en)
+            d = descs[i]
+            d.offset, d.dtype = off, 0 if cal is None else 1
+            if cal is not None:
+                d.cal_range, d.cal_offset, d.cal_digit = cal
+            if en > len(sig) or rd_st >= en:
+                out[i] = Alignment(rid_, RD_EN_PAST_END if en > len(sig) else SKIP_REASONS[7])
+                d.n_samples = 0
+            else:
+                part = sig[rd_st:en]
+                parts.append(part)
+                d.n_samples = len(part)
+                off += len(part)
+        dtypes = {descs[i].dtype for i in range(n)}
+        if len(dtypes) > 1:
+            raise ValueError("one batch holds one signal type")
+        samples = np.concatenate(parts) if parts else np.zeros(1, np.float32)
+        samples = np.ascontiguousarray(samples, dtype=np.int16 if dtypes == {1} else np.float32)
+        res = (DtwAlignResult * max(n, 1))()
+        N.check(self._L.unc_dtw_align_batch(self._h, n, descs, samples.ctypes.data, qs, 1 if paths else 0, res))
+        for i in range(n):
+            if out[i] is not None:
+                continue
+            r = res[i]
+            kw = dict(n_events=r.n_events, n_kept=r.n_kept)
+            if r.status:
+                out[i] = Alignment(queries[i][0], SKIP_REASONS[r.status], **kw)
+                continue
+            kw.update(score=float(r.score), mean_score=float(r.mean_score))
+            if paths:
+                p = np.zeros((r.path_len, 2), np.uint64)
+                m = np.zeros(max(r.n_kept, 1), np.float32)
+                k = np.zeros(max(qs[i].rf_en - qs[i].rf_st - 4, 1), np.uint16)
+                N.check(self._L.unc_dtw_align_path(self._h, i, p.ctypes.data, m.ctypes.data, k.ctypes.data))
+                kw.update(path=p[::-1].copy(), means=m[:r.n_kept], kmers=k[:qs[i].rf_en - qs[i].rf_st - 4])
+            out[i] = Alignment(queries[i][0], **kw)
+        return out
+
+    def last_times(self):
+        """CUDA-event times of the last batch in ms: h2d, events, mask, kmers, target, norm, sweep, total; then the
+        number of sweep launches and of matrix cells."""
+        ms = np.zeros(8, np.float32)
+        la, ce = C.c_uint64(), C.c_uint64()
+        N.check(self._L.unc_dtw_align_last_times(self._h, ms.ctypes.data, C.byref(la), C.byref(ce)))
+        keys = ("h2d", "events", "mask", "kmers", "target", "norm", "sweep", "total")
+        return dict(zip(keys, (float(x) for x in ms))), la.value, ce.value
+
+
+def r94d_cost(kmer, mean):
+    """DTWr94d's cost of (k-mer, event mean) as the reference's dtw_test driver compiles it: the float abs of the float
+    difference (the driver includes <math.h> before dtw.hpp)."""
+    lv = model_table()[0::2]
+    return np.abs(np.asarray(mean, np.float32) - lv[np.asarray(kmer, dtype=np.int64)].astype(np.float32)).astype(np.float32)
+
+
+def format_path(a):
+    """The lines of the path file of an Alignment (print_path, src/dtw.hpp:135-143): event index, k-mer index, the
+    k-mer of the row, the mean of the column and their cost, each followed by a tab."""
+    ev, km = a.path[:, 0].astype(np.int64), a.path[:, 1].astype(np.int64)
+    k = a.kmers[km]
+    m = a.means[ev]
+    c = r94d_cost(k, m)
+    return "".join("%d\t%d\t%d\t%g\t%g\t\n" % (e, r, kk, float(mm), float(cc)) for e, r, kk, mm, cc in zip(ev, km, k, m, c))
+
+
+class QueryError(ValueError):
+    pass
+
+
+def load_queries(fname, aligner):
+    """load_queries (src/dtw_test.cpp:27-58): `rd_name rd_st rd_en rf_name rf_st rf_en strand` per line, keyed by read
+    name (a later line for a read replaces an earlier one).  Returns {read name: (rd_st, rd_en, contig, rf_st, rf_en,
+    fwd)}.  A malformed line, an unknown contig or a strand other than + / - rejects the whole file (QueryError)."""
+    out = {}
+    with open(fname) as f:
+        for ln, line in enumerate(f, 1):
+            fields = line.split()
+            if not fields:
+                continue
+            where = "%s:%d: " % (fname, ln)
+            if len(fields) != 7:
+                raise QueryError(where + "expected 7 fields (rd_name rd_st rd_en rf_name rf_st rf_en strand), got %d" % len(fields))
+            name, rd_st, rd_en, contig, rf_st, rf_en, strand = fields
+            try:
+                nums = [int(x, 10) for x in (rd_st, rd_en, rf_st, rf_en)]
+            except ValueError:
+                raise QueryError(where + "coordinates must be non-negative integers") from None
+            if min(nums) < 0 or max(nums[:2]) >= 1 << 32 or max(nums[2:]) >= 1 << 64:
+                raise QueryError(where + "coordinates must be non-negative integers")
+            if strand not in ("+", "-"):
+                raise QueryError(where + "strand must be + or -, got %r" % strand)
+            if aligner.contig(contig) is None:
+                raise QueryError(where + "unknown contig %r" % contig)
+            out[name] = (nums[0], nums[1], contig, nums[2], nums[3], strand == "+")
+    return out
+
+
+def host_skip(aligner, n_signal, rd_st, rd_en, contig, rf_st, rf_en):
+    """The reason a query is skipped before the device, or None (unc_dtw_align_batch applies the same checks)."""
+    en = n_signal if rd_en == 0 else rd_en
+    if en > n_signal:
+        return RD_EN_PAST_END
+    if rd_st >= en:
+        return SKIP_REASONS[7]
+    rid, ln = aligner.contig(contig)
+    if rf_en > ln or rf_st > rf_en:
+        return SKIP_REASONS[5]
+    if rf_en - rf_st < 5:
+        return SKIP_REASONS[6]
+    return None
