@@ -842,8 +842,7 @@ struct K2V2 {              // the worker warps' per-event state (unc_k2v2.cuh)
     u32 koff[UNC_NKMER];   // bucket start in the sorted key array
     u32 kagg[UNC_NKMER];   // (gap sources | child seeds << 16) of the bucket, then their exclusive prefix
     u32 fresh_cand[32], fresh_mask[32], fresh_before[32];   // fresh-source candidates / plan per 32-k-mer word
-    u32 grab[2];           // bucket hand-out counters (sort pass, emit pass)
-    u32 n_units;           // 32-key chunks of large buckets listed for the emit pass (W.elist)
+    u32 grab;              // bucket hand-out counter (sort + walk pass)
     u16 mfirst[K2V2_MAX_MERGED];   // per merged-group k-mer: gap sources of its bucket before its first run (0xFFFF: no run)
 #if defined(UNC_PHASE_TIMING) && !defined(UNC_EMUL)
     u32 pt_dur[4][K2_MAXSEG];      // phase-timing builds: every worker warp's own time in B / C2 / D1 / E of the event
@@ -977,7 +976,7 @@ UNC_DEV long long pt_clock() { long long v; asm volatile("mov.u64 %0, %%clock64;
 #define PT_WB pt_w0 = pt_clock();
 #define PT_WE(ph) if (lane == 0) v2->pt_dur[ph][ww] = (u32) (pt_clock() - pt_w0);
 #define PT_WARR(ph) if (lane == 0) v2->pt_dur[ph][ww] = (u32) pt_clock(); w_sync(); s_atomic_max(&v2->pt_dur[ph][ww], (u32) pt_clock());   /* arrival of the warp's last lane at the barrier that follows */
-#define PT_WREL(ph) if (lane == 0 && *(volatile u32 *) &v2->grab[0] != 0xFFFFFFFFu) { const long long _t = pt_clock(); v2->pt_dur[ph][ww] = (u32) _t; PT_TRACE(event_i, 30, _t) }      /* the warp's release from the barrier before */
+#define PT_WREL(ph) if (lane == 0 && *(volatile u32 *) &v2->grab != 0xFFFFFFFFu) { const long long _t = pt_clock(); v2->pt_dur[ph][ww] = (u32) _t; PT_TRACE(event_i, 30, _t) }      /* the warp's release from the barrier before */
 #define PT_WLAG(ph, s_last, s_first) if (wt == 0) { const u32 _now = (u32) pt_clock(); u32 _mn = 0xFFFFFFFFu, _mx = 0; for (u32 _w = 0; _w < nwk; _w++) { \
         const u32 _d = _now - *(volatile u32 *) &v2->pt_dur[ph][_w]; _mn = _d < _mn ? _d : _mn; _mx = _d > _mx ? _d : _mx; } pt_acc[s_last] += _mn; pt_acc[s_first] += _mx; }
 #define PT_WTRK(ph, s) if (wt == 0) pt_acc[s] += (u32) pt_clock() - *(volatile u32 *) &v2->pt_dur[ph][K2_MAXSEG - 2 + (event_i & 1u)];
