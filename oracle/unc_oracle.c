@@ -840,11 +840,44 @@ typedef struct {
     tracker_t trk;
     u32 path_mask, path_tail_move;
     orc_paf_rec *rec;
+    orc_trace_seed *tseeds;    /* orc_set_path_trace: the event's seeds so far */
+    u32 tseeds_n, tseeds_cap;
 } mapper_t;
 
 static orc_trace_fn g_trace = NULL;
 static void *g_trace_ud = NULL;
 void orc_set_trace(orc_trace_fn fn, void *ud) { g_trace = fn; g_trace_ud = ud; }
+static orc_path_trace_fn g_path_trace = NULL;
+static void *g_path_trace_ud = NULL;
+void orc_set_path_trace(orc_path_trace_fn fn, void *ud) { g_path_trace = fn; g_path_trace_ud = ud; }
+
+static void trace_seed(mapper_t *mp, u64 ref_end, u32 move_count, u32 evt) {
+    if (mp->tseeds_n == mp->tseeds_cap) {
+        mp->tseeds_cap = mp->tseeds_cap ? 2 * mp->tseeds_cap : 256;
+        mp->tseeds = (orc_trace_seed *) realloc(mp->tseeds, (size_t) mp->tseeds_cap * sizeof(orc_trace_seed));
+    }
+    orc_trace_seed *s = &mp->tseeds[mp->tseeds_n++];
+    s->ref_end = ref_end; s->move_count = move_count; s->evt = evt;
+}
+
+static void path_trace(mapper_t *mp, u32 nn) {
+    orc_trace_row *rows = (orc_trace_row *) calloc((size_t) nn + 1, sizeof(orc_trace_row));
+    for (u32 i = 0; i < nn; i++) {
+        const path_t *q = &mp->prev[i];
+        orc_trace_row *o = &rows[i];
+        if (q->length == 0) continue;
+        o->fm_start = q->fm_start; o->fm_end = q->fm_end;
+        o->kmer = q->kmer; o->length = q->length; o->consec_stays = q->consec_stays; o->sa_checked = q->sa_checked;
+        o->event_moves = q->event_moves;
+        memcpy(&o->seed_prob, &q->seed_prob, 4);
+        memcpy(&o->prob_sum, &q->prob_sums[q->length], 4);
+        o->valid = 1;
+    }
+    u32 flags[ORC_NKMER / 32] = {0};
+    for (u32 k = 0; k < ORC_NKMER; k++) if (mp->sources_added[k]) flags[k >> 5] |= 1u << (k & 31u);
+    g_path_trace(g_path_trace_ud, mp->event_i, nn, rows, mp->tseeds_n, mp->tseeds, flags);
+    free(rows);
+}
 
 /* reference src/mapper.cpp:751-772 (make_source) */
 static void make_source(path_t *q, u64 st, u64 en, u16 kmer, float prob) {
@@ -903,6 +936,7 @@ static void update_seeds(mapper_t *mp, path_t *q, int path_ended) {
     for (u64 s = q->fm_start; s <= q->fm_end; s++) {
         u64 sa_end = mp->idx->seq_len - orc_sa(mp->idx, s);
         trk_add_seed(&mp->trk, mp->prm, sa_end, move_count, mp->event_i - (u32) path_ended);
+        if (g_path_trace) trace_seed(mp, sa_end, move_count, mp->event_i - (u32) path_ended);
         mp->rec->n_seeds++;
     }
 }
@@ -1184,6 +1218,7 @@ static int map_next_event(mapper_t *mp, float event, float mean_event_len) {
     const float *probs = mp->kmer_probs;
     const float source_prob = x->thresh[0];
     const u32 maxp = prm->max_paths;
+    mp->tseeds_n = 0;
 
     u32 nn = 0; /* next_path - next_paths_.begin() */
 
@@ -1301,6 +1336,7 @@ static int map_next_event(mapper_t *mp, float event, float mean_event_len) {
         }
         g_trace(g_trace_ud, mp->event_i, nn, mp->trk.n, h);
     }
+    if (g_path_trace) path_trace(mp, nn);
 
     cluster_t sc = trk_get_final(&mp->trk, prm);
     if (sc.evt_st <= sc.evt_en) {
@@ -1327,6 +1363,7 @@ static void mapper_free(mapper_t *mp) {
     free(mp->next);
     free(mp->trk.set);
     free(mp->trk.lens);
+    free(mp->tseeds);
 }
 
 /* reference src/mapper.cpp:188-200 (map_read), :216-246 (reset), read_buffer.cpp:263-266 */

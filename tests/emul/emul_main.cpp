@@ -144,6 +144,51 @@ extern "C" int emu_dtw_batch(const float *model_means_stdvs, int cost_kind, int 
     return 0;
 }
 
+// The mapper's per-event trace in the oracle's row layout (orc_trace_row / orc_trace_seed of oracle/unc_oracle.h), so
+// that a test compares the path buffers of both sides byte for byte.  item = the batch index, or the channel when streaming.
+struct EmuTraceRow {
+    uint64_t fm_start, fm_end;
+    uint32_t kmer, length, consec_stays, sa_checked, event_moves, seed_prob, prob_sum, valid;
+};
+struct EmuTraceSeed {
+    uint64_t ref_end;
+    uint32_t move_count, evt;
+};
+typedef void (*EmuPathTraceFn)(void *ud, uint32_t item, uint32_t event_i, uint32_t nn, const EmuTraceRow *rows, uint32_t n_seeds,
+                               const EmuTraceSeed *seeds, const uint32_t *flags, uint32_t overflow);
+static EmuPathTraceFn g_trace_fn = nullptr;
+static void *g_trace_ud = nullptr;
+static void emu_path_trace_decode(u32 item, u32 event_i, u32 nn, const uint4 *recs, const u32 *order, u32 n_rows,
+                                  const uint2 *rl, const u32 *flags, u32 overflow) {
+    std::vector<EmuTraceRow> rows(nn + 1);
+    memset(rows.data(), 0, rows.size() * sizeof(EmuTraceRow));
+    for (u32 i = 0; i < nn; i++) {
+        if (order[i] & UNC_INVALID) continue;               // a dup: invalidated at its position
+        const uint4 q0 = recs[(size_t) order[i] * 2], q1 = recs[(size_t) order[i] * 2 + 1];
+        EmuTraceRow &o = rows[i];
+        o.fm_start = q0.x; o.fm_end = q0.y;
+        o.kmer = q0.z & UNC_KMASK; o.length = (q0.z >> 16) & 0xFFu; o.consec_stays = (q0.z >> 24) & 0xFFu;
+        o.event_moves = q0.w & UNC_PATH_MASK; o.sa_checked = q0.w >> 31;
+        o.seed_prob = q1.x; o.prob_sum = q1.y; o.valid = 1;
+    }
+    std::vector<EmuTraceSeed> seeds(n_rows + 1);
+    for (u32 j = 0; j < n_rows; j++) {
+        seeds[j].ref_end = rl[j].x; seeds[j].move_count = rl[j].y & 0xFFu;
+        seeds[j].evt = (rl[j].y & 0x100u) ? event_i - 1u : event_i;
+    }
+    if (g_trace_fn) g_trace_fn(g_trace_ud, item, event_i, nn, rows.data(), n_rows, seeds.data(), flags, overflow);
+}
+extern "C" void emu_set_path_trace(EmuPathTraceFn fn, void *ud) {
+    g_trace_fn = fn; g_trace_ud = ud;
+    g_emu_path_trace = fn ? emu_path_trace_decode : nullptr;
+}
+// how often the bucket phases met each of their edges (K2S_* of unc_device.cuh), since the last reset
+extern "C" uint32_t emu_k2_shape_stats(unsigned long *out, int reset) {
+    if (out) memcpy(out, g_emu_k2_shape, sizeof(g_emu_k2_shape));
+    if (reset) memset(g_emu_k2_shape, 0, sizeof(g_emu_k2_shape));
+    return K2S_N;
+}
+
 extern "C" void emu_set_tie_order(int mode) { g_tie_order = mode; }
 extern "C" void emu_tie_stats(unsigned long *out, int reset) {
     out[0] = g_emu_tie_stats[0]; out[1] = g_emu_tie_stats[1];
@@ -229,7 +274,7 @@ static int emu_map_batch_impl(void *pidx, const unc_params *prm, const unc_read_
     std::vector<uint2> hist((size_t) 24 * (nchmax * 160 + maxp));
     std::vector<u32> order((size_t) 2 * maxp);
     std::vector<uint4> clu((size_t) max_blocks * 32 * 2), dir(max_blocks + 1);
-    const u32 rl_cap = 16384;
+    const u32 rl_cap = UNC_RL_CAP;
     std::vector<uint2> rlist(2 * rl_cap);
     DevWork W;
     W.paths = paths.data(); W.hist = hist.data(); W.wlist = wlist.data(); W.ckey = ckey.data(); W.cks = cks.data(); W.elist = elist.data(); W.order = order.data(); W.rlist = rlist.data();
@@ -327,7 +372,7 @@ void *emu_stream_create(void *pidx, const unc_params *prm, uint32_t n_channels, 
     DevWorkStrides &S = T->S;
     S.paths = 2 * (nchmax * 160 + maxp) * 2; S.hist = 24 * (nchmax * 160 + maxp); S.ckey = 2 * maxp;
     S.cks = nchmax * 160; S.elist = nchmax * 32; S.order = 2 * maxp;
-    const u32 rl_cap = 16384;
+    const u32 rl_cap = UNC_RL_CAP;
     S.rlist = 2 * rl_cap; S.clu = (size_t) max_blocks * 32 * 2; S.dir = (size_t) max_blocks + 1;
     T->paths.resize(n * S.paths); T->hist.resize(n * S.hist); T->ckey.resize(n * S.ckey); T->cks.resize(n * S.cks);
     T->wlist.resize(n * S.cks); T->elist.resize(n * S.elist); T->order.resize(n * S.order); T->rlist.resize(n * S.rlist);

@@ -77,6 +77,25 @@ def build():
 
 _lib = None
 
+# emu_set_path_trace's callback: (ud, item, event_i, nn, rows, n_seeds, seeds, flags[32], overflow); rows and seeds in the
+# layout of orclib.TRACE_ROW / orclib.TRACE_SEED (oracle/unc_oracle.h orc_trace_row / orc_trace_seed)
+PATH_TRACE_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p,
+                            C.c_void_p, C.c_uint32)
+
+# the counters of emu_k2_shape_stats, in their order (K2S_* of uncalled_b200/csrc/unc_device.cuh)
+K2_SHAPES = ("pack", "pack_full", "large", "huge", "merged_small", "merged_big", "merged_cross",
+             "pass0", "pass1", "pass2", "pass3", "pass4", "eq_run", "eq_run_cross", "dup_cross",
+             "cut_in_chunk", "cut_at_chunk", "full_exact", "room_cut", "recount")
+
+
+def k2_shape_stats(reset=False):
+    """{shape: count} of the bucket phases' edges met since the last reset (emulator builds only)."""
+    n = lib().emu_k2_shape_stats(None, 0)
+    assert n == len(K2_SHAPES), n
+    a = (C.c_ulong * n)()
+    lib().emu_k2_shape_stats(a, 1 if reset else 0)
+    return dict(zip(K2_SHAPES, (int(v) for v in a)))
+
 
 def _bind(L):
     """argtypes of one loaded emulator library"""
@@ -107,6 +126,10 @@ def _bind(L):
     L.emu_stream_step.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_int]
     L.emu_stream_norm_state.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
     L.emu_stream_norm_state.restype = C.c_uint64
+    L.emu_set_path_trace.argtypes = [PATH_TRACE_FN, C.c_void_p]
+    L.emu_set_path_trace.restype = None
+    L.emu_k2_shape_stats.argtypes = [C.c_void_p, C.c_int]
+    L.emu_k2_shape_stats.restype = C.c_uint32
     return L
 
 

@@ -76,6 +76,15 @@ def build_oracle():
         subprocess.run(["make", "-C", ORACLE_DIR, "ref"], check=True, capture_output=True)
 
 
+# orc_set_path_trace (oracle/unc_oracle.h): one row per path buffer position, one entry per seed of the event
+TRACE_ROW = np.dtype([("fm_start", "<u8"), ("fm_end", "<u8"), ("kmer", "<u4"), ("length", "<u4"), ("consec_stays", "<u4"),
+                      ("sa_checked", "<u4"), ("event_moves", "<u4"), ("seed_prob", "<u4"), ("prob_sum", "<u4"),
+                      ("valid", "<u4")])
+TRACE_SEED = np.dtype([("ref_end", "<u8"), ("move_count", "<u4"), ("evt", "<u4")])
+assert TRACE_ROW.itemsize == 48 and TRACE_SEED.itemsize == 16
+# (ud, event_i, n_paths, rows, n_seeds, seeds, sources_added[32])
+PATH_TRACE_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p)
+
 _orc = None
 
 
@@ -120,6 +129,8 @@ def orc():
                                                C.POINTER(C.c_uint32), C.POINTER(C.c_int32)]
         lib.orc_stream_map_channel_norm.argtypes = lib.orc_stream_map_channel.argtypes + [C.c_void_p, C.c_void_p]
         lib.orc_stream_chunk_pushes.argtypes = [C.POINTER(OrcParams), f32p, C.c_uint32, C.c_uint32, u32p]
+        lib.orc_set_path_trace.argtypes = [PATH_TRACE_FN, C.c_void_p]
+        lib.orc_set_path_trace.restype = None
         _orc = lib
     return _orc
 

@@ -461,7 +461,7 @@ int unc_pool_create(const unc_index *idx, const unc_params *prm, uint32_t max_re
     uint64_t ev_cap = std::min<uint64_t>(prm->max_events, longest / 3 + 16);
     uint64_t mb = std::max<uint64_t>(1024, ev_cap * 2);
     mb = std::min<uint64_t>(mb, 1u << 17);
-    const size_t rl_cap = 64 * 1024;   // seed rows of one event (typically tens)
+    const size_t rl_cap = UNC_RL_CAP;
     size_t per_slot = (P->paths_stride + P->ckey_stride + 2 * P->cks_stride + P->elist_stride) * 16 + P->hist_stride * 8 + P->order_stride * 4 + 2 * rl_cap * 8 + mb * (UNC_BLK * 32 + 16);
     size_t free_b = 0, total_b = 0;
     PT(cudaMemGetInfo(&free_b, &total_b));

@@ -120,6 +120,8 @@ struct DevBatch {
     u32 *flags_out = nullptr;
 };
 
+#define UNC_RL_CAP (64u * 1024u)   /* seed rows of one event (typically tens): DevWork::rl_cap of every slot */
+
 struct DevWork {   // per-slot (per-CTA) workspaces; slot s uses [s*stride, (s+1)*stride)
     uint4 *paths;      // 2 generations x (ceil(max_paths/32)*160 chunk-local child slots + max_paths sources) x 2 uint4
     uint2 *hist;       // 24 generations x the same record index space: (cumulative log-prob C, parent record index)
@@ -600,6 +602,15 @@ UNC_DEV void trk_erase(Tracker &t, u32 d, u32 pos) {
     t.n_live--;
     if (cnt == 0) {
         trk_dir_close(t, d);
+        // keep the store dense (n_alloc == nb): the last block moves into the freed one.  Without this, every block that
+        // empties is lost, and a read whose clusters churn for long exhausts max_blocks with few of them alive.
+        const u32 last = --t.n_alloc;
+        if (blk != last) {
+            for (u32 i = (u32) lane; i < UNC_BLK * 2u; i += 32u) t.blocks[(size_t) blk * UNC_BLK * 2u + i] = t.blocks[(size_t) last * UNC_BLK * 2u + i];
+            for (u32 i = (u32) lane; i < t.nb; i += 32u)
+                if (t.dir[i].z == last) t.dir[i].z = blk;
+            w_sync();
+        }
     } else {
         // new first key: entry that is now at slot 0
         u32 src = pos == 0 ? 1u : 0u;
@@ -873,6 +884,30 @@ struct K2Shared {          // per CTA
 #include "unc_pdqsort.cuh"
 #ifdef UNC_EMUL
 static unsigned long g_emu_tie_stats[2];   // test statistics of the exact-ties path (emulator builds only)
+// Emulator builds only: worker thread 0 hands every COMMITTED event to this hook: the generation just written (records
+// and order), the seed rows the tracker takes, the sources_added_ words and the overflow flag (tests/emul/emul_main.cpp).
+typedef void (*UncEmuPathTrace)(u32 item, u32 event_i, u32 nn, const uint4 *recs, const u32 *order, u32 n_rows,
+                                const uint2 *rows, const u32 *flags, u32 overflow);
+static UncEmuPathTrace g_emu_path_trace;
+// ... and counts how often the bucket phases meet their edges (emu_k2_shape_stats)
+enum {
+    K2S_PACK, K2S_PACK_FULL,                  // packs of small buckets; packs holding exactly 32 keys
+    K2S_LARGE, K2S_HUGE,                      // single-k-mer buckets of 33..256 keys; of more than 256
+    K2S_MERGED_SMALL, K2S_MERGED_BIG,         // merged groups' buckets of <= 32 keys; of more
+    K2S_MERGED_CROSS,                         // a merged walk's window ends on a dup or a k-mer run that goes on behind it
+    K2S_PASS0, K2S_PASS1, K2S_PASS2, K2S_PASS3, K2S_PASS4,   // radix passes of k2v2_sort_big (odd: the copy home)
+    K2S_EQ_RUN, K2S_EQ_RUN_CROSS,             // runs of equal fm_start in a radix-sorted bucket; such a run across 32 keys
+    K2S_DUP_CROSS,                            // a dup pair across two 32-key passes of the carried walk
+    K2S_CUT_IN_CHUNK, K2S_CUT_AT_CHUNK,       // max_paths cuts the children inside a chunk; between two chunks
+    K2S_FULL_EXACT,                           // the children fill the buffer exactly (no cut)
+    K2S_ROOM_CUT,                             // phase E: the fresh sources of a word fill the buffer
+    K2S_RECOUNT,                              // EXACT: buckets walked again on the pdqsort order
+    K2S_N
+};
+static unsigned long g_emu_k2_shape[K2S_N];
+#define K2S_IF(cond, i) { if (cond) g_emu_k2_shape[i]++; }
+#else
+#define K2S_IF(cond, i)
 #endif
 // PathBuffer::make_source (reference src/mapper.cpp:751-772): prob_sums_ = {0, prob}
 UNC_DEV void write_source(uint4 *rec, uint2 *hist_e, u32 idx, u32 st, u32 en, u32 kmer, float prob) {

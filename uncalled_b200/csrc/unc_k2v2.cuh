@@ -91,6 +91,7 @@ UNC_DEV void k2v2_sort_big(uint4 *keys, uint4 *tmp, u32 o, u32 n, u32 lo, u32 sp
     const int lane = w_lane();
     const u32 lt = w_lanemask_lt();
     const u32 npass = (span_bits + 7u) >> 3;
+    K2S_IF(lane == 0, K2S_PASS0 + npass)
     uint4 *src = keys + o, *dst = tmp + o;
     const u32 nch = (n + 31u) >> 5;
     for (u32 pass = 0; pass < npass; pass++) {
@@ -144,6 +145,8 @@ UNC_DEV void k2v2_sort_big(uint4 *keys, uint4 *tmp, u32 o, u32 n, u32 lo, u32 sp
         if (head) {
             u32 e = g + 1;
             while (e < n && src[e].x == s) e++;
+            K2S_IF(true, K2S_EQ_RUN)
+            K2S_IF(e > (c + 1u) * 32u, K2S_EQ_RUN_CROSS)
             for (u32 i = g + 1; i < e; i++) {
                 const uint4 key = src[i];
                 u32 j = i;
@@ -334,6 +337,7 @@ UNC_DEV u32 k2v2_walk_merged(K2Shared *sh, const uint4 *keys, uint4 *verd, u32 n
             }
             if (cur.w & 1u) { fl |= K2V2_V_SEED; nseed++; }
         }
+        K2S_IF(j == 31u && has_next && ((fl & K2V2_V_DUP) || ((nxt.w >> 6) & 0xFFu) == sub), K2S_MERGED_CROSS)
         verd[i] = k2v2_verdict(src_st, src_en, before, fl, kmer, slot);
     }
     w_sync();
@@ -391,6 +395,7 @@ UNC_DEV bool k2v2_exact_order(K2Shared *sh, const DevWork &W, u32 nc, u32 maxp, 
     if (wt == 0) v2->grab = 0;
     for (u32 m = wt; m < K2V2_MAX_MERGED; m += nwt) v2->mfirst[m] = 0xFFFFu;
     c_sync_sub(1, (int) nwt);
+    K2S_IF(wt == 0, K2S_RECOUNT)
     return true;
 }
 
@@ -683,7 +688,15 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
         if (wt == 0) sh->wl_cnt = 0;
         const u32 nc_total = nch_prev ? sh->bc[2] : 0u;
         const u32 nc = nc_total < maxp ? nc_total : maxp;
+        K2S_IF(wt == 0 && nc_total == maxp, K2S_FULL_EXACT)
         if (nc_total > maxp) {
+#ifdef UNC_EMUL
+            if (wt == 0) {
+                bool at_chunk = false;
+                for (u32 c = 0; c < nch_prev; c++) at_chunk |= sh->bcnt[c] == maxp;
+                g_emu_k2_shape[at_chunk ? K2S_CUT_AT_CHUNK : K2S_CUT_IN_CHUNK]++;
+            }
+#endif
             // the cap cut the children (chunk order = emission order): take the dropped ones -- emission index >= max_paths,
             // all in the last chunks -- out of the bucket counts instead of counting everything again.  kagg is still zero.
             for (u32 c = ww; c < nch_prev; c += nwk) {
@@ -775,6 +788,7 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
                         const int l = d_ffs(todo_m) - 1;
                         todo_m &= todo_m - 1;
                         const u32 o = w_shfl(bo, l), n = w_shfl(bn, l), moff = w_shfl(meta, l) >> 8;
+                        K2S_IF(lane == 0 && sort, n <= 32u ? K2S_MERGED_SMALL : K2S_MERGED_BIG)
                         if (sort && n <= 32u) k2v2_sort_small(ckA + o, n, (uint4 *) stage_r);
                         else if (sort) {
                             u32 lo = 0xFFFFFFFFu, hi = 0;
@@ -793,6 +807,7 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
                         todo &= todo - 1;
                         const u32 o = w_shfl(bo, l), n = w_shfl(bn, l);
                         const u32 kmer = v2->t.gkmer[grp * 32u + (u32) l], slot = (u32) l * 32u + grp;
+                        K2S_IF(lane == 0 && sort, n > 256u ? K2S_HUGE : K2S_LARGE)
                         const uint2 kr = tb->kmer_range[kmer];
                         const bool prob_ok = sh->probs[kmer] >= source_prob;
                         if (sort) {   // span of the bucket's fm_start values -> radix passes
@@ -812,6 +827,7 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
                             u32 mxo;
                             const K2V2Walk wk = k2v2_walk(cur, nx, ny, a, has_next, g == 0, g == 0, g0 != 0, carry_mx, prob_ok, kr, &mxo);
                             carry_mx = mxo;
+                            K2S_IF(a && wk.dup && lane == 31, K2S_DUP_CROSS)
                             if (a) {
                                 const u32 src_b = n_src + (u32) d_popc(wk.m_b & lt) + (u32) d_popc(wk.m_a & lt), seed_b = n_seed + (u32) d_popc(wk.m_seed & lt);
                                 ckB[o + g] = k2v2_verdict(wk.as, wk.ae, src_b | (seed_b << 16), k2v2_flags(wk), kmer, slot);
@@ -828,6 +844,8 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
                     u32 remaining = w_ballot(cnt != 0);
                     while (remaining) {
                         const K2V2Pack pk = k2v2_next_pack(cnt, P, &remaining);
+                        K2S_IF(lane == 0 && sort, K2S_PACK)
+                        K2S_IF(lane == 31 && pk.a && sort, K2S_PACK_FULL)
                         const u32 addr = w_shfl(bo, (int) pk.bl) + pk.pos;
                         uint4 k = make_uint4(0, 0, 0, 0);
                         if (pk.a) k = ckA[addr];
@@ -995,6 +1013,7 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
             const u32 room = maxp - before;
             u32 visited = 0xFFFFFFFFu;
             if ((u32) d_popc(m_add) >= room) {
+                K2S_IF(lane == 0, K2S_ROOM_CUT)
                 // the room-th add fills the buffer; k-mers after it are never visited
                 u32 mm = m_add;
                 for (u32 q = 1; q < room; q++) mm &= mm - 1;
@@ -1030,6 +1049,12 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
             break;
         }
         if (wt == 0) { k2v2_add64(sh->tot_children, nc); k2v2_add64(sh->tot_sources, nn - nc); }
+#ifdef UNC_EMUL
+        if (wt == 0 && g_emu_path_trace)
+            g_emu_path_trace(STREAM ? B.chan[r] : r, event_i, nn, W.paths + (size_t) (gen ^ 1u) * gen_recs * 2,
+                             W.order + (size_t) (gen ^ 1u) * maxp, n_rows, W.rlist + (size_t) (event_i & 1u) * W.rl_cap,
+                             sh->flags, sh->wk_overflow);
+#endif
         my_blocks += pend_blocks; my_steps += pend_steps;
         pend_blocks = pend_steps = 0;
         prev_size = nn;
