@@ -406,6 +406,12 @@ int unc_mask_external(const char *full_fasta, const char *target_fasta, uint32_t
 float unc_mask_external_last_kernel_ms(void);
 void unc_mask_external_last_times(float ms[4], uint64_t *h2d_bytes);
 
+/* ---- resource accounting (tests) -----------------------------------------------------------------------------
+ * What the library holds at this moment: bytes of device memory, bytes of pinned host memory, and CUDA streams plus
+ * events.  An object's free call, or the end of a call that holds nothing past its return, gives back what it took.
+ * The DTW workspace stays held between unc_dtw_batch / unc_dtw_align_batch calls until unc_dtw_release. */
+int unc_debug_held(uint64_t *device_bytes, uint64_t *pinned_bytes, uint32_t *handles);
+
 /* ---- fast5 input (host; no libhdf5 needed) -------------------------------------------------------------
  *   unc_fast5_open      Fast5Reader::open_next: format detection and the list of reads
  *                                                      src/fast5_reader.cpp:134-177

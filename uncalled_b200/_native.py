@@ -88,7 +88,8 @@ EXPORTS = ["unc_strerror", "unc_last_error", "unc_device_count", "unc_init", "un
            "unc_mask_internal", "unc_mask_last_kernel_ms", "unc_mask_external", "unc_mask_external_last_kernel_ms",
            "unc_mask_external_last_times", "unc_index_build_device", "unc_index_build_device_last_times",
            "unc_index_build_device_last_active", "unc_dtw_aligner_create", "unc_dtw_aligner_free", "unc_dtw_aligner_contig",
-           "unc_dtw_aligner_set_budget", "unc_dtw_align_batch", "unc_dtw_align_path", "unc_dtw_align_last_times"]
+           "unc_dtw_aligner_set_budget", "unc_dtw_align_batch", "unc_dtw_align_path", "unc_dtw_align_last_times",
+           "unc_debug_held"]
 
 
 def build(force=False, verbose=False):
@@ -216,6 +217,7 @@ def lib():
     L.unc_dtw_align_batch.argtypes = [vp, u32, vp, vp, vp, C.c_int, vp]
     L.unc_dtw_align_path.argtypes = [vp, u32, vp, vp, vp]
     L.unc_dtw_align_last_times.argtypes = [vp, vp, C.POINTER(u64), C.POINTER(u64)]
+    L.unc_debug_held.argtypes = [C.POINTER(u64), C.POINTER(u64), C.POINTER(u32)]
     _lib = L
     return L
 

@@ -6,9 +6,12 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <atomic>
 #include <chrono>
+#include <memory>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "unc_device.cuh"
@@ -183,47 +186,166 @@ static int fail(int code, const std::string &msg) {
             return fail(UNC_E_CUDA, std::string(#x) + ": " + cudaGetErrorString(_e));                  \
     } while (0)
 
+// Checks that a CUDA device exists and makes `device` current: the first device step of every entry point that has
+// no index or pool to take its device from.
+static int use_device(int device) {
+    int n = 0;
+    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0)
+        return fail(UNC_E_NO_DEVICE, "no CUDA device (the product has no CPU fallback)");
+    if (device < 0 || device >= n) return fail(UNC_E_ARG, "device out of range");
+    CUDA_TRY(cudaSetDevice(device));
+    return UNC_OK;
+}
+
+// ------------------------------------------------------------------ resource owners
+// Every device buffer, pinned buffer, stream and event the library holds belongs to one of these owners, which releases
+// it in its destructor.  A failed allocation leaves the owner empty and clears the runtime's last error, so a later
+// cudaGetLastError() does not report it as a launch failure.  What the owners hold is counted (unc_debug_held).
+
+static std::atomic<uint64_t> g_held_device{0}, g_held_pinned{0};
+static std::atomic<uint32_t> g_held_handles{0};
+
+// n elements of T from cudaMalloc (DevMem) or cudaMallocHost (PinnedMem)
+template <typename T, bool PINNED>
+struct CudaMem {
+    T *p = nullptr;
+    size_t n = 0;
+
+    CudaMem() = default;
+    CudaMem(CudaMem &&o) noexcept { *this = std::move(o); }
+    CudaMem &operator=(CudaMem &&o) noexcept { std::swap(p, o.p); std::swap(n, o.n); return *this; }
+    ~CudaMem() { reset(); }
+    operator T *() const { return p; }
+    size_t bytes() const { return n * sizeof(T); }
+
+    cudaError_t reset() {
+        if (!p) return cudaSuccess;
+        const cudaError_t e = PINNED ? cudaFreeHost(p) : cudaFree(p);
+        (PINNED ? g_held_pinned : g_held_device) -= bytes();
+        p = nullptr; n = 0;
+        return e;
+    }
+    // frees what the owner holds, then allocates count elements; on failure the owner stays empty
+    cudaError_t try_alloc(size_t count) {
+        reset();
+        const cudaError_t e = PINNED ? cudaMallocHost((void **) &p, count * sizeof(T)) : cudaMalloc((void **) &p, count * sizeof(T));
+        if (e != cudaSuccess) { p = nullptr; cudaGetLastError(); return e; }
+        n = count;
+        (PINNED ? g_held_pinned : g_held_device) += bytes();
+        return cudaSuccess;
+    }
+    int alloc(size_t count, const char *what) {
+        const cudaError_t e = try_alloc(count);
+        if (e != cudaSuccess) return fail(UNC_E_CUDA, std::string(PINNED ? "cudaMallocHost " : "cudaMalloc ") + what + ": " + cudaGetErrorString(e));
+        return UNC_OK;
+    }
+    // reallocates only when count is larger than what is held; the contents are not kept
+    int grow(size_t count, const char *what) { return count <= n ? UNC_OK : alloc(count, what); }
+    // bytes from the host, followed by pad zero bytes
+    int upload(const void *src, size_t bytes, size_t pad, const char *what) {
+        if (int rc = alloc((bytes + pad + sizeof(T) - 1) / sizeof(T), what)) return rc;
+        if (pad) CUDA_TRY(cudaMemset((char *) p + bytes, 0, pad));
+        CUDA_TRY(cudaMemcpy(p, src, bytes, cudaMemcpyHostToDevice));
+        return UNC_OK;
+    }
+};
+template <typename T> using DevMem = CudaMem<T, false>;
+template <typename T> using PinnedMem = CudaMem<T, true>;
+
+// a non-blocking stream (CudaStream) or an event (CudaEvent)
+template <typename H>
+struct CudaHandle {
+    static constexpr bool STREAM = std::is_same<H, cudaStream_t>::value;
+    H h = nullptr;
+
+    CudaHandle() = default;
+    CudaHandle(CudaHandle &&o) noexcept { std::swap(h, o.h); }
+    ~CudaHandle() {
+        if (!h) return;
+        if constexpr (STREAM) cudaStreamDestroy(h); else cudaEventDestroy(h);
+        g_held_handles--;
+    }
+    operator H() const { return h; }
+    int create() {
+        if constexpr (STREAM) CUDA_TRY(cudaStreamCreateWithFlags(&h, cudaStreamNonBlocking)); else CUDA_TRY(cudaEventCreate(&h));
+        g_held_handles++;
+        return UNC_OK;
+    }
+};
+using CudaStream = CudaHandle<cudaStream_t>;
+using CudaEvent = CudaHandle<cudaEvent_t>;
+
+// The mapper's per-slot workspaces (DevWork) for n slots: array a of slot s starts at s * strides.a.
+struct DevWorkMem {
+    DevMem<uint4> paths, ckey, wlist, cks, elist, clu, dir;
+    DevMem<uint2> hist, rlist;
+    DevMem<u32> order;
+
+    // allocates every array (the history zeroed) and points W's arrays at them
+    int alloc(size_t n, const DevWorkStrides &S, DevWork &W) {
+        int rc;
+        if ((rc = paths.alloc(n * S.paths, "paths")) || (rc = ckey.alloc(n * S.ckey, "ckey")) || (rc = hist.alloc(n * S.hist, "hist")))
+            return rc;
+        CUDA_TRY(cudaMemset(hist, 0, hist.bytes()));
+        if ((rc = wlist.alloc(n * S.cks, "wlist")) || (rc = cks.alloc(n * S.cks, "cks")) || (rc = elist.alloc(n * S.elist, "elist")) ||
+            (rc = order.alloc(n * S.order, "order")) || (rc = rlist.alloc(n * S.rlist, "rlist")) ||
+            (rc = clu.alloc(n * S.clu, "clu")) || (rc = dir.alloc(n * S.dir, "dir")))
+            return rc;
+        W.paths = paths; W.hist = hist; W.wlist = wlist; W.ckey = ckey; W.cks = cks;
+        W.elist = elist; W.order = order; W.rlist = rlist; W.clu = clu; W.dir = dir;
+        return UNC_OK;
+    }
+};
+
 struct unc_index {
     HostIndex h;
     DevIndex ix;
     int device = 0;
     std::vector<uint2> kmer_range;  // host copy
-    void *d_bwt = nullptr, *d_sa = nullptr, *d_kr = nullptr, *d_model = nullptr, *d_thresh = nullptr;
-    void *d_seq_off = nullptr, *d_seq_len = nullptr, *d_sa_full = nullptr, *d_occ2 = nullptr, *d_krank = nullptr;
+    DevMem<u32> d_bwt, d_sa, d_seq_len, d_sa_full;
+    DevMem<uint2> d_kr;
+    DevMem<float> d_model, d_thresh;
+    DevMem<u64> d_seq_off;
+    DevMem<uint4> d_occ2;
+    DevMem<K2V2Tab> d_krank;
     size_t device_bytes = 0;
 };
 
 struct unc_pool {
+    CudaStream stream;           // first, so that it is destroyed after everything queued on it
     const unc_index *idx = nullptr;
     unc_params prm;
     DevParams dp;
     uint32_t max_reads = 0;
     uint64_t max_samples = 0;
-    uint32_t ev_stride = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // [5]: end of k1_events
+    uint32_t ev_stride = 0;      // floats per read of d_events and d_normed; 0 while neither is allocated
+    CudaEvent ev[6];             // [5]: end of k1_events
     // batch buffers
-    void *d_samples = nullptr;
-    DevReadDesc *d_reads = nullptr, *h_reads = nullptr;
-    float *d_events = nullptr, *d_normed = nullptr, *d_scale = nullptr, *d_shift = nullptr, *d_mel = nullptr;
-    u32 *d_n_events = nullptr, *d_queue = nullptr, *d_k1_flags = nullptr;   // d_queue: [k2 queue, k1 queue, 4 x k1 stats]
+    DevMem<char> d_samples;
+    DevMem<DevReadDesc> d_reads;
+    PinnedMem<DevReadDesc> h_reads;
+    DevMem<float> d_events, d_normed, d_scale, d_shift, d_mel;
+    DevMem<u32> d_n_events, d_queue, d_k1_flags;   // d_queue: [k2 queue, k1 queue, 4 x k1 stats]
     uint32_t k1_grid = 0;
-    DevRec *d_out = nullptr;
-    unsigned long long *d_dbg = nullptr;
-    unc_paf_rec *h_out = nullptr;  // pinned staging
+    DevMem<DevRec> d_out;
+    DevMem<unsigned long long> d_dbg;
+    PinnedMem<unc_paf_rec> h_out;  // staging
     // workspaces
+    DevWorkMem work;
     DevWork W;
-    size_t paths_stride = 0, hist_stride = 0, ckey_stride = 0, cks_stride = 0, elist_stride = 0, order_stride = 0, rlist_stride = 0, clu_stride = 0, dir_stride = 0;
+    DevWorkStrides S{};
     uint32_t n_slots = 0, grid = 0;
     size_t smem = 0;
     unc_timing last;
-    cudaEvent_t ev_user[2] = {nullptr, nullptr};   // unc_pool_record / unc_pool_elapsed
+    CudaEvent ev_user[2];        // unc_pool_record / unc_pool_elapsed
     uint32_t pending_n = 0;      // reads of a submitted, not yet collected batch (unc_map_batch_submit / _wait)
     uint64_t pending_h2d = 0;
     // ordered mode (unc_map_batch_ordered): per-read sources_added_ words in / out, allocated on first use
     int tie_order = 0;           // unc_pool_set_tie_order: 0 = emission order (k2_map), 1 = the reference's pdqsort (k2_map_exact)
-    u32 *d_flags_in = nullptr, *d_flags_out = nullptr, *d_cand = nullptr;
+    DevMem<u32> d_flags_in, d_flags_out, d_cand;
     bool want_cand = false;      // the next batch_enqueue also launches k_event0_cands
+
+    ~unc_pool() { if (stream) cudaStreamSynchronize(stream); }
 };
 
 extern "C" {
@@ -251,11 +373,7 @@ int unc_device_count(void) {
 }
 
 int unc_init(int device) {
-    int n = 0;
-    cudaError_t e = cudaGetDeviceCount(&n);
-    if (e != cudaSuccess || n == 0) return fail(UNC_E_NO_DEVICE, "no CUDA device (the product has no CPU fallback)");
-    if (device < 0 || device >= n) return fail(UNC_E_ARG, "device out of range");
-    CUDA_TRY(cudaSetDevice(device));
+    if (int rc = use_device(device)) return rc;
     g_device = device;
     return UNC_OK;
 }
@@ -278,59 +396,41 @@ int unc_params_default(unc_params *p) {
     return UNC_OK;
 }
 
-static int upload(void **dst, const void *src, size_t bytes, size_t pad, size_t *total) {
-    CUDA_TRY(cudaMalloc(dst, bytes + pad));
-    if (pad) CUDA_TRY(cudaMemset((char *) *dst + bytes, 0, pad));
-    CUDA_TRY(cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice));
-    *total += bytes + pad;
-    return UNC_OK;
-}
-
 int unc_index_load(const char *bwa_prefix, const char *preset, const char *model_table_path, unc_index **out) {
     if (!bwa_prefix || !out || !model_table_path) return fail(UNC_E_ARG, "null argument");
-    int n = 0;
-    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0)
-        return fail(UNC_E_NO_DEVICE, "no CUDA device (the product has no CPU fallback)");
-    CUDA_TRY(cudaSetDevice(g_device));
-    unc_index *x = new unc_index();
+    if (int rc = use_device(g_device)) return rc;
+    std::unique_ptr<unc_index> x(new unc_index());
     x->device = g_device;
-    if (!hix_load_model(x->h, model_table_path) || !hix_load(x->h, bwa_prefix, preset ? preset : "default")) {
-        std::string e = x->h.error;
-        delete x;
-        return fail(UNC_E_IO, e);
-    }
+    if (!hix_load_model(x->h, model_table_path) || !hix_load(x->h, bwa_prefix, preset ? preset : "default"))
+        return fail(UNC_E_IO, x->h.error);
     HostIndex &h = x->h;
-    if (h.seq_len >= 0xFFFFFF00ull) {
-        delete x;
+    if (h.seq_len >= 0xFFFFFF00ull)
         return fail(UNC_E_TOO_LARGE, "FM index longer than 2^32 rows is not supported by the u32 device image");
-    }
-    int rc;
-#define UP(dst, src, bytes, pad) if ((rc = upload(&(dst), (src), (bytes), (pad), &x->device_bytes)) != UNC_OK) { unc_index_free(x); return rc; }
-    UP(x->d_bwt, h.bwt.data(), h.bwt.size() * 4, 64);
-    UP(x->d_sa, h.sa32.data(), h.sa32.size() * 4, 16);
     std::vector<float> model(3 * 1024);
     std::copy(h.lv_mean.begin(), h.lv_mean.end(), model.begin());
     std::copy(h.lv_var2.begin(), h.lv_var2.end(), model.begin() + 1024);
     std::copy(h.lognorm.begin(), h.lognorm.end(), model.begin() + 2048);
-    UP(x->d_model, model.data(), model.size() * 4, 0);
-    UP(x->d_thresh, h.thresh, 64 * 4, 0);
     std::vector<u64> so(h.offsets.begin(), h.offsets.end());
     if (so.empty()) so.push_back(0);
     std::vector<u32> sl(h.lens.begin(), h.lens.end());
     if (sl.empty()) sl.push_back(0);
-    UP(x->d_seq_off, so.data(), so.size() * 8, 0);
-    UP(x->d_seq_len, sl.data(), sl.size() * 4, 0);
-#undef UP
-    if (cudaMalloc(&x->d_kr, 1024 * sizeof(uint2)) != cudaSuccess) { unc_index_free(x); return fail(UNC_E_CUDA, "cudaMalloc kmer ranges"); }
-    x->device_bytes += 1024 * sizeof(uint2);
+    int rc;
+    if ((rc = x->d_bwt.upload(h.bwt.data(), h.bwt.size() * 4, 64, "bwt")) ||
+        (rc = x->d_sa.upload(h.sa32.data(), h.sa32.size() * 4, 16, "sampled suffix array")) ||
+        (rc = x->d_model.upload(model.data(), model.size() * 4, 0, "pore model")) ||
+        (rc = x->d_thresh.upload(h.thresh, 64 * 4, 0, "thresholds")) ||
+        (rc = x->d_seq_off.upload(so.data(), so.size() * 8, 0, "sequence offsets")) ||
+        (rc = x->d_seq_len.upload(sl.data(), sl.size() * 4, 0, "sequence lengths")) ||
+        (rc = x->d_kr.alloc(1024, "kmer ranges")))
+        return rc;
     DevIndex &ix = x->ix;
-    ix.bwt = (const uint4 *) x->d_bwt;
-    ix.sa = (const u32 *) x->d_sa;
-    ix.kmer_range = (const uint2 *) x->d_kr;
-    ix.lv_mean = (const float *) x->d_model;
+    ix.bwt = (const uint4 *) (u32 *) x->d_bwt;
+    ix.sa = x->d_sa;
+    ix.kmer_range = x->d_kr;
+    ix.lv_mean = x->d_model;
     ix.lv_var2 = ix.lv_mean + 1024;
     ix.lognorm = ix.lv_mean + 2048;
-    ix.thresh = (const float *) x->d_thresh;
+    ix.thresh = x->d_thresh;
     ix.primary = (u32) h.primary;
     ix.seq_len = (u32) h.seq_len;
     for (int i = 0; i < 5; i++) ix.L2[i] = (u32) h.L2[i];
@@ -339,34 +439,33 @@ int unc_index_load(const char *bwa_prefix, const char *preset, const char *model
     ix.occ2 = nullptr; ix.kt = nullptr;
     {   // expanded suffix array (4 bytes per FM row); skipped when device memory is short
         size_t free_b = 0, total_b = 0;
-        const size_t need = ((size_t) h.seq_len + 1) * 4;
-        if (!getenv("UNC_NO_SA_EXPAND") && cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && need < free_b / 4 &&
-            cudaMalloc(&x->d_sa_full, need) == cudaSuccess) {
-            u32 n_rows = (u32) h.seq_len + 1u;
-            k_sa_expand<<<(n_rows + 255) / 256, 256>>>(ix, (u32 *) x->d_sa_full, n_rows);
-            if (cudaDeviceSynchronize() == cudaSuccess) { ix.sa_full = (const u32 *) x->d_sa_full; x->device_bytes += need; }
-            else { unc_index_free(x); return fail(UNC_E_CUDA, "k_sa_expand failed"); }
+        const u32 n_rows = (u32) h.seq_len + 1u;
+        if (!getenv("UNC_NO_SA_EXPAND") && cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && (size_t) n_rows * 4 < free_b / 4 &&
+            x->d_sa_full.try_alloc(n_rows) == cudaSuccess) {
+            k_sa_expand<<<(n_rows + 255) / 256, 256>>>(ix, x->d_sa_full, n_rows);
+            if (cudaDeviceSynchronize() != cudaSuccess) return fail(UNC_E_CUDA, "k_sa_expand failed");
+            ix.sa_full = x->d_sa_full;
         }
     }
-    k_kmer_ranges<<<4, 256>>>(ix, (uint2 *) x->d_kr);
+    k_kmer_ranges<<<4, 256>>>(ix, x->d_kr);
     x->kmer_range.resize(1024);
     cudaError_t e = cudaMemcpy(x->kmer_range.data(), x->d_kr, 1024 * sizeof(uint2), cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { unc_index_free(x); return fail(UNC_E_CUDA, std::string("k_kmer_ranges: ") + cudaGetErrorString(e)); }
+    if (e != cudaSuccess) return fail(UNC_E_CUDA, std::string("k_kmer_ranges: ") + cudaGetErrorString(e));
     {   // GPU-side layouts of the mapper's worker warps: 32-byte Occ blocks, k-mer rank tables
         const u32 n_blk = (u32) (h.bwt.size() / 16) * 2u;
-        if (cudaMalloc(&x->d_occ2, (size_t) n_blk * 32 + 64) != cudaSuccess) { unc_index_free(x); return fail(UNC_E_CUDA, "cudaMalloc occ2"); }
-        cudaMemset((char *) x->d_occ2 + (size_t) n_blk * 32, 0, 64);
-        k_occ2_build<<<(n_blk + 255) / 256, 256>>>(ix.bwt, (uint4 *) x->d_occ2, n_blk);
+        if ((rc = x->d_occ2.alloc((size_t) n_blk * 2 + 4, "occ2"))) return rc;
+        cudaMemset(x->d_occ2 + (size_t) n_blk * 2, 0, 64);
+        k_occ2_build<<<(n_blk + 255) / 256, 256>>>(ix.bwt, x->d_occ2, n_blk);
         K2V2Tab kt;
-        if (!hix_k2v2_tab(x->kmer_range.data(), kt)) { unc_index_free(x); return fail(UNC_E_TOO_LARGE, "more overlapping k-mer FM ranges than the bucket table holds"); }
-        if (cudaMalloc(&x->d_krank, sizeof(kt)) != cudaSuccess ||
-            cudaMemcpy(x->d_krank, &kt, sizeof(kt), cudaMemcpyHostToDevice) != cudaSuccess ||
-            cudaDeviceSynchronize() != cudaSuccess) { unc_index_free(x); return fail(UNC_E_CUDA, "occ2 / k-mer bucket tables"); }
-        ix.occ2 = (const uint4 *) x->d_occ2;
-        ix.kt = (const K2V2Tab *) x->d_krank;
-        x->device_bytes += (size_t) n_blk * 32 + 64 + sizeof(kt);
+        if (!hix_k2v2_tab(x->kmer_range.data(), kt)) return fail(UNC_E_TOO_LARGE, "more overlapping k-mer FM ranges than the bucket table holds");
+        if ((rc = x->d_krank.upload(&kt, sizeof(kt), 0, "k-mer bucket tables"))) return rc;
+        if (cudaDeviceSynchronize() != cudaSuccess) return fail(UNC_E_CUDA, "occ2 / k-mer bucket tables");
+        ix.occ2 = x->d_occ2;
+        ix.kt = x->d_krank;
     }
-    *out = x;
+    x->device_bytes = x->d_bwt.bytes() + x->d_sa.bytes() + x->d_model.bytes() + x->d_thresh.bytes() + x->d_seq_off.bytes() +
+                      x->d_seq_len.bytes() + x->d_kr.bytes() + x->d_sa_full.bytes() + x->d_occ2.bytes() + x->d_krank.bytes();
+    *out = x.release();
     return UNC_OK;
 }
 
@@ -400,12 +499,7 @@ int unc_index_thresholds(const unc_index *x, float out[64]) {
     return UNC_OK;
 }
 
-void unc_index_free(unc_index *x) {
-    if (!x) return;
-    cudaFree(x->d_bwt); cudaFree(x->d_sa); cudaFree(x->d_kr); cudaFree(x->d_model); cudaFree(x->d_thresh);
-    cudaFree(x->d_seq_off); cudaFree(x->d_seq_len); cudaFree(x->d_sa_full); cudaFree(x->d_occ2); cudaFree(x->d_krank);
-    delete x;
-}
+void unc_index_free(unc_index *x) { delete x; }
 
 int unc_pool_create(const unc_index *idx, const unc_params *prm, uint32_t max_reads, uint64_t max_samples,
                     unc_pool **out) {
@@ -413,48 +507,48 @@ int unc_pool_create(const unc_index *idx, const unc_params *prm, uint32_t max_re
     std::string err;
     if (unc_check_params(*prm, err)) return fail(UNC_E_ARG, err);
     CUDA_TRY(cudaSetDevice(idx->device));
-    unc_pool *P = new unc_pool();
+    std::unique_ptr<unc_pool> P(new unc_pool());
     P->idx = idx;
     P->prm = *prm;
     P->dp = unc_make_dev_params(*prm, idx->h);
     P->max_reads = max_reads;
     P->max_samples = max_samples;
     memset(&P->last, 0, sizeof(P->last));
-    int rc = UNC_OK;
-    auto bail = [&](int code, const std::string &m) { unc_pool_free(P); return fail(code, m); };
-#define PT(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) return bail(UNC_E_CUDA, std::string(#x) + ": " + cudaGetErrorString(_e)); } while (0)
-    PT(cudaStreamCreateWithFlags(&P->stream, cudaStreamNonBlocking));
-    for (int i = 0; i < 6; i++) PT(cudaEventCreate(&P->ev[i]));
+    int rc;
+    if ((rc = P->stream.create())) return rc;
+    for (int i = 0; i < 6; i++)
+        if ((rc = P->ev[i].create())) return rc;
     cudaDeviceProp prop;
-    PT(cudaGetDeviceProperties(&prop, idx->device));
+    CUDA_TRY(cudaGetDeviceProperties(&prop, idx->device));
     P->smem = K2_SMEM_BYTES(prm->max_paths);
-    PT(raise_dyn_smem(k2_map, P->smem));
+    CUDA_TRY(raise_dyn_smem(k2_map, P->smem));
     int per_sm = 0;
-    PT(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k2_map, K2_THREADS, P->smem));
-    if (per_sm < 1) return bail(UNC_E_CUDA, "k2_map does not fit on an SM");
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k2_map, K2_THREADS, P->smem));
+    if (per_sm < 1) return fail(UNC_E_CUDA, "k2_map does not fit on an SM");
     if (const char *e = getenv("UNC_K2_CTAS_PER_SM")) { int v = atoi(e); if (v >= 1 && v < per_sm) per_sm = v; }   // tuning knob
     uint32_t grid = (uint32_t) prop.multiProcessorCount * (uint32_t) per_sm;
     if (grid > max_reads) grid = max_reads;
     {
         const size_t k1_smem = (size_t) K1_WARPS * sizeof(K1WarpSmem);
-        PT(raise_dyn_smem(k1_events, k1_smem));
+        CUDA_TRY(raise_dyn_smem(k1_events, k1_smem));
         int k1_per_sm = 0;
-        PT(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k1_per_sm, k1_events, K1_WARPS * 32, k1_smem));
-        if (k1_per_sm < 1) return bail(UNC_E_CUDA, "k1_events does not fit on an SM");
+        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k1_per_sm, k1_events, K1_WARPS * 32, k1_smem));
+        if (k1_per_sm < 1) return fail(UNC_E_CUDA, "k1_events does not fit on an SM");
         P->k1_grid = (uint32_t) prop.multiProcessorCount * (uint32_t) k1_per_sm;
     }
     // per-slot workspace sizes
     const size_t maxp = prm->max_paths;
     const size_t nchmax = (maxp + 31) / 32;
-    P->paths_stride = 2 * (nchmax * 160 + maxp) * 2;   // uint4: chunk-local child slots + sources, two generations
-    P->hist_stride = 24 * (nchmax * 160 + maxp);      // uint2: (C, parent) per record index, 24 generations
-    P->ckey_stride = 2 * maxp;        // uint4
-    P->cks_stride = nchmax * 160;     // uint4
-    P->elist_stride = nchmax * 32;    // uint4
-    P->order_stride = 2 * maxp;       // u32
+    DevWorkStrides &S = P->S;
+    S.paths = 2 * (nchmax * 160 + maxp) * 2;   // uint4: chunk-local child slots + sources, two generations
+    S.hist = 24 * (nchmax * 160 + maxp);      // uint2: (C, parent) per record index, 24 generations
+    S.ckey = 2 * maxp;        // uint4
+    S.cks = nchmax * 160;     // uint4
+    S.elist = nchmax * 32;    // uint4
+    S.order = 2 * maxp;       // u32
     if (const char *e = getenv("UNC_K2_SLOT_PAD")) {   // experiment knob: spread the slots over a larger address span
         size_t f = (size_t) atoi(e);
-        if (f >= 2 && f <= 8) { P->paths_stride *= f; P->hist_stride *= f; P->ckey_stride *= f; P->cks_stride *= f; P->elist_stride *= f; P->order_stride *= f; }
+        if (f >= 2 && f <= 8) { S.paths *= f; S.hist *= f; S.ckey *= f; S.cks *= f; S.elist *= f; S.order *= f; }
     }
     uint64_t longest = max_samples < 0xFFFFFFFFull ? max_samples : 0xFFFFFFFFull;
     // seed clusters: at most a few per event in practice; blocks are >= half full after splits
@@ -462,66 +556,43 @@ int unc_pool_create(const unc_index *idx, const unc_params *prm, uint32_t max_re
     uint64_t mb = std::max<uint64_t>(1024, ev_cap * 2);
     mb = std::min<uint64_t>(mb, 1u << 17);
     const size_t rl_cap = UNC_RL_CAP;
-    size_t per_slot = (P->paths_stride + P->ckey_stride + 2 * P->cks_stride + P->elist_stride) * 16 + P->hist_stride * 8 + P->order_stride * 4 + 2 * rl_cap * 8 + mb * (UNC_BLK * 32 + 16);
+    size_t per_slot = (S.paths + S.ckey + 2 * S.cks + S.elist) * 16 + S.hist * 8 + S.order * 4 + 2 * rl_cap * 8 + mb * (UNC_BLK * 32 + 16);
     size_t free_b = 0, total_b = 0;
-    PT(cudaMemGetInfo(&free_b, &total_b));
+    CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
     size_t fixed = max_samples * 4 + (size_t) max_reads * (sizeof(DevReadDesc) + sizeof(DevRec) + 20) + (64u << 20);
-    P->ev_stride = 0;
-    if (free_b < fixed + per_slot) return bail(UNC_E_NOMEM, "not enough device memory for the pool");
+    if (free_b < fixed + per_slot) return fail(UNC_E_NOMEM, "not enough device memory for the pool");
     size_t budget = (size_t) ((free_b - fixed) * 0.85);
     while ((size_t) grid * per_slot > budget && grid > 1) grid--;
     P->grid = grid;
     P->n_slots = grid;
-    P->rlist_stride = 2 * rl_cap;
+    S.rlist = 2 * rl_cap;
     P->W.rl_cap = (u32) rl_cap;
-    P->clu_stride = (size_t) mb * UNC_BLK * 2;
-    P->dir_stride = (size_t) mb + 1;
+    S.clu = (size_t) mb * UNC_BLK * 2;
+    S.dir = (size_t) mb + 1;
     P->W.max_blocks = (u32) mb;
-    PT(cudaMalloc(&P->W.paths, (size_t) P->n_slots * P->paths_stride * 16));
-    PT(cudaMalloc(&P->W.ckey, (size_t) P->n_slots * P->ckey_stride * 16));
-    PT(cudaMalloc(&P->W.hist, (size_t) P->n_slots * P->hist_stride * 8));
-    PT(cudaMemset(P->W.hist, 0, (size_t) P->n_slots * P->hist_stride * 8));
-    PT(cudaMalloc(&P->W.wlist, (size_t) P->n_slots * P->cks_stride * 16));
-    PT(cudaMalloc(&P->W.cks, (size_t) P->n_slots * P->cks_stride * 16));
-    PT(cudaMalloc(&P->W.elist, (size_t) P->n_slots * P->elist_stride * 16));
-    PT(cudaMalloc(&P->W.order, (size_t) P->n_slots * P->order_stride * 4));
-    PT(cudaMalloc(&P->W.rlist, (size_t) P->n_slots * P->rlist_stride * 8));
-    PT(cudaMalloc(&P->W.clu, (size_t) P->n_slots * P->clu_stride * 16));
-    PT(cudaMalloc(&P->W.dir, (size_t) P->n_slots * P->dir_stride * 16));
-    PT(cudaMalloc(&P->d_samples, max_samples * 4 + 64));
-    PT(cudaMalloc(&P->d_reads, (size_t) max_reads * sizeof(DevReadDesc)));
-    PT(cudaMallocHost(&P->h_reads, (size_t) max_reads * sizeof(DevReadDesc)));
-    PT(cudaMalloc(&P->d_scale, (size_t) max_reads * 4));
-    PT(cudaMalloc(&P->d_shift, (size_t) max_reads * 4));
-    PT(cudaMalloc(&P->d_mel, (size_t) max_reads * 4));
-    PT(cudaMalloc(&P->d_n_events, (size_t) max_reads * 4));
-    PT(cudaMalloc(&P->d_queue, 32));
-    PT(cudaMalloc(&P->d_k1_flags, (size_t) max_reads * 4));
-    PT(cudaMalloc(&P->d_out, (size_t) max_reads * sizeof(DevRec)));
+    if ((rc = P->work.alloc(P->n_slots, S, P->W)) ||
+        (rc = P->d_samples.alloc(max_samples * 4 + 64, "sample staging")) ||
+        (rc = P->d_reads.alloc(max_reads, "read descriptors")) ||
+        (rc = P->h_reads.alloc(max_reads, "read descriptors")) ||
+        (rc = P->d_scale.alloc(max_reads, "scale")) ||
+        (rc = P->d_shift.alloc(max_reads, "shift")) ||
+        (rc = P->d_mel.alloc(max_reads, "mean event length")) ||
+        (rc = P->d_n_events.alloc(max_reads, "event counts")) ||
+        (rc = P->d_queue.alloc(8, "queues")) ||
+        (rc = P->d_k1_flags.alloc(max_reads, "k1 flags")) ||
+        (rc = P->d_out.alloc(max_reads, "records")))
+        return rc;
 #ifdef UNC_PHASE_TIMING
-    PT(cudaMalloc(&P->d_dbg, (size_t) max_reads * 512 + UNC_PT_TRACE_BYTES));     // counters per read, then the timeline of one read
-    PT(cudaMemset(P->d_dbg, 0, (size_t) max_reads * 512 + UNC_PT_TRACE_BYTES));
+    // counters per read, then the timeline of one read
+    if ((rc = P->d_dbg.alloc(((size_t) max_reads * 512 + UNC_PT_TRACE_BYTES) / 8, "phase timing"))) return rc;
+    CUDA_TRY(cudaMemset(P->d_dbg, 0, P->d_dbg.bytes()));
 #endif
-    PT(cudaMallocHost(&P->h_out, (size_t) max_reads * sizeof(unc_paf_rec)));
-#undef PT
-    (void) rc;
-    *out = P;
+    if ((rc = P->h_out.alloc(max_reads, "records"))) return rc;
+    *out = P.release();
     return UNC_OK;
 }
 
-void unc_pool_free(unc_pool *P) {
-    if (!P) return;
-    cudaFree(P->W.paths); cudaFree(P->W.hist); cudaFree(P->W.wlist); cudaFree(P->W.ckey); cudaFree(P->W.cks); cudaFree(P->W.elist); cudaFree(P->W.order); cudaFree(P->W.rlist); cudaFree(P->W.clu); cudaFree(P->W.dir);
-    cudaFree(P->d_samples); cudaFree(P->d_reads); cudaFreeHost(P->h_reads);
-    cudaFree(P->d_events); cudaFree(P->d_normed);
-    cudaFree(P->d_scale); cudaFree(P->d_shift); cudaFree(P->d_mel); cudaFree(P->d_n_events); cudaFree(P->d_queue); cudaFree(P->d_k1_flags);
-    cudaFree(P->d_out); cudaFreeHost(P->h_out); cudaFree(P->d_dbg);
-    cudaFree(P->d_flags_in); cudaFree(P->d_flags_out); cudaFree(P->d_cand);
-    for (int i = 0; i < 2; i++) if (P->ev_user[i]) cudaEventDestroy(P->ev_user[i]);
-    for (int i = 0; i < 6; i++) if (P->ev[i]) cudaEventDestroy(P->ev[i]);
-    if (P->stream) cudaStreamDestroy(P->stream);
-    delete P;
-}
+void unc_pool_free(unc_pool *P) { delete P; }
 
 // validates descriptors, stages them, (re)allocates the events buffer; returns the sample span
 static int stage_reads(unc_pool *P, const unc_read_desc *reads, uint32_t n, uint64_t *span_bytes, uint32_t *max_n,
@@ -544,15 +615,14 @@ static int stage_reads(unc_pool *P, const unc_read_desc *reads, uint32_t n, uint
     *max_n = mx;
     uint32_t stride = (mx + 3u) & ~3u;
     if (stride == 0) stride = 4;
-    if (stride > P->ev_stride || (want_normed && !P->d_normed)) {
-        if (stride > P->ev_stride) {
-            cudaFree(P->d_events); P->d_events = nullptr;
-            cudaFree(P->d_normed); P->d_normed = nullptr;
-            P->ev_stride = stride;
-            CUDA_TRY(cudaMalloc(&P->d_events, (size_t) P->max_reads * P->ev_stride * 4));
-        }
-        if (want_normed && !P->d_normed) CUDA_TRY(cudaMalloc(&P->d_normed, (size_t) P->max_reads * P->ev_stride * 4));
+    int rc;
+    if (stride > P->ev_stride) {
+        P->ev_stride = 0;
+        P->d_normed.reset();
+        if ((rc = P->d_events.grow((size_t) P->max_reads * stride, "events buffer"))) return rc;
+        P->ev_stride = stride;
     }
+    if (want_normed && (rc = P->d_normed.grow((size_t) P->max_reads * P->ev_stride, "normalised events buffer"))) return rc;
     return UNC_OK;
 }
 
@@ -566,15 +636,15 @@ static DevBatch make_batch(unc_pool *P, const void *d_samples, uint64_t samples_
     B.reads = P->d_reads;
     B.n_reads = n;
     B.events = P->d_events;
-    B.normed = normed ? P->d_normed : nullptr;
+    B.normed = normed ? (float *) P->d_normed : nullptr;
     B.ev_stride = P->ev_stride;
     B.n_events = P->d_n_events;
     B.scale = P->d_scale; B.shift = P->d_shift; B.mean_event_len = P->d_mel;
     B.queue = P->d_queue;
     B.dbg = P->d_dbg;
     B.out = P->d_out;
-    B.seq_offsets = (const u64 *) P->idx->d_seq_off;
-    B.seq_lens = (const u32 *) P->idx->d_seq_len;
+    B.seq_offsets = P->idx->d_seq_off;
+    B.seq_lens = P->idx->d_seq_len;
     B.n_seqs = (u32) P->idx->h.names.size();
     B.l_pac = (u64) P->idx->h.l_pac;
     return B;
@@ -616,11 +686,12 @@ static int batch_enqueue(unc_pool *P, const unc_read_desc *reads, uint32_t n, co
     // the pool's own staging buffer is padded, so whole 16-byte bulk copies may run past `span`
     DevBatch B = make_batch(P, d_samples, on_device ? span : ((span + 15) & ~(uint64_t) 15), n, false);
     if (h_flags_in) {
-        if (!P->d_flags_in) {
-            CUDA_TRY(cudaMalloc(&P->d_flags_in, (size_t) P->max_reads * 128));
-            CUDA_TRY(cudaMalloc(&P->d_flags_out, (size_t) P->max_reads * 128));
-            CUDA_TRY(cudaMalloc(&P->d_cand, (size_t) P->max_reads * 128));
+        if (!P->d_cand) {   // allocated last, so it stands for all three
             CUDA_TRY(raise_dyn_smem(k2_map_ord, P->smem));
+            if ((rc = P->d_flags_in.alloc((size_t) P->max_reads * 32, "ordered-mode flags")) ||
+                (rc = P->d_flags_out.alloc((size_t) P->max_reads * 32, "ordered-mode flags")) ||
+                (rc = P->d_cand.alloc((size_t) P->max_reads * 32, "ordered-mode candidates")))
+                return rc;
         }
         CUDA_TRY(cudaMemcpyAsync(P->d_flags_in, h_flags_in, (size_t) n * 128, cudaMemcpyHostToDevice, s));
         B.flags_in = P->d_flags_in;
@@ -632,17 +703,16 @@ static int batch_enqueue(unc_pool *P, const unc_read_desc *reads, uint32_t n, co
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaEventRecord(P->ev[2], s));
     uint32_t grid = std::min<uint32_t>(P->grid, n);
+    const DevWorkStrides &S = P->S;
     if (P->tie_order)
-        k2_map_exact<<<grid, K2_THREADS, P->smem, s>>>(P->idx->ix, P->dp, B, P->W, P->paths_stride, P->hist_stride, P->ckey_stride,
-                                                       P->cks_stride, P->elist_stride, P->order_stride, P->rlist_stride,
-                                                       P->clu_stride, P->dir_stride);
+        k2_map_exact<<<grid, K2_THREADS, P->smem, s>>>(P->idx->ix, P->dp, B, P->W, S.paths, S.hist, S.ckey, S.cks, S.elist, S.order,
+                                                       S.rlist, S.clu, S.dir);
     else if (h_flags_in)
-        k2_map_ord<<<grid, K2_THREADS, P->smem, s>>>(P->idx->ix, P->dp, B, P->W, P->paths_stride, P->hist_stride, P->ckey_stride,
-                                                     P->cks_stride, P->elist_stride, P->order_stride, P->rlist_stride,
-                                                     P->clu_stride, P->dir_stride);
+        k2_map_ord<<<grid, K2_THREADS, P->smem, s>>>(P->idx->ix, P->dp, B, P->W, S.paths, S.hist, S.ckey, S.cks, S.elist, S.order,
+                                                     S.rlist, S.clu, S.dir);
     else
-        k2_map<<<grid, K2_THREADS, P->smem, s>>>(P->idx->ix, P->dp, B, P->W, P->paths_stride, P->hist_stride, P->ckey_stride, P->cks_stride,
-                                                 P->elist_stride, P->order_stride, P->rlist_stride, P->clu_stride, P->dir_stride);
+        k2_map<<<grid, K2_THREADS, P->smem, s>>>(P->idx->ix, P->dp, B, P->W, S.paths, S.hist, S.ckey, S.cks, S.elist, S.order,
+                                                 S.rlist, S.clu, S.dir);
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaEventRecord(P->ev[3], s));
     CUDA_TRY(cudaMemcpyAsync(P->h_out, P->d_out, (size_t) n * sizeof(DevRec), cudaMemcpyDeviceToHost, s));
@@ -701,7 +771,8 @@ int unc_map_batch_wait(unc_pool *P, unc_paf_rec *out) {
 int unc_pool_record(unc_pool *P, int slot) {
     if (!P || slot < 0 || slot > 1) return fail(UNC_E_ARG, "bad argument");
     CUDA_TRY(cudaSetDevice(P->idx->device));
-    if (!P->ev_user[slot]) CUDA_TRY(cudaEventCreate(&P->ev_user[slot]));
+    if (!P->ev_user[slot])
+        if (int rc = P->ev_user[slot].create()) return rc;
     CUDA_TRY(cudaEventRecord(P->ev_user[slot], P->stream));
     return UNC_OK;
 }
@@ -811,12 +882,10 @@ int unc_events_batch(unc_pool *P, const unc_read_desc *reads, uint32_t n, const 
 int unc_match_probs(const unc_index *x, float event, float out[1024]) {
     if (!x || !out) return fail(UNC_E_ARG, "null argument");
     CUDA_TRY(cudaSetDevice(x->device));
-    float *d = nullptr;
-    CUDA_TRY(cudaMalloc(&d, 1024 * 4));
+    DevMem<float> d;
+    if (int rc = d.alloc(1024, "match probabilities")) return rc;
     k_match_probs<<<4, 256>>>(x->ix, event, d);
-    cudaError_t e = cudaMemcpy(out, d, 1024 * 4, cudaMemcpyDeviceToHost);
-    cudaFree(d);
-    if (e != cudaSuccess) return fail(UNC_E_CUDA, cudaGetErrorString(e));
+    CUDA_TRY(cudaMemcpy(out, d, 1024 * 4, cudaMemcpyDeviceToHost));
     return UNC_OK;
 }
 
@@ -824,31 +893,27 @@ int unc_fm_neighbors(const unc_index *x, uint32_t n, const uint64_t *start, cons
                      uint64_t *ostart, uint64_t *oend) {
     if (!x || !n) return fail(UNC_E_ARG, "null argument");
     CUDA_TRY(cudaSetDevice(x->device));
-    u64 *ds, *de, *dos, *doe;
-    u8 *db;
-    CUDA_TRY(cudaMalloc(&ds, n * 8)); CUDA_TRY(cudaMalloc(&de, n * 8)); CUDA_TRY(cudaMalloc(&dos, n * 8));
-    CUDA_TRY(cudaMalloc(&doe, n * 8)); CUDA_TRY(cudaMalloc(&db, n));
-    cudaMemcpy(ds, start, n * 8, cudaMemcpyHostToDevice);
-    cudaMemcpy(de, end, n * 8, cudaMemcpyHostToDevice);
-    cudaMemcpy(db, base, n, cudaMemcpyHostToDevice);
+    DevMem<u64> ds, de, dos, doe;
+    DevMem<u8> db;
+    int rc;
+    if ((rc = ds.upload(start, n * 8, 0, "start rows")) || (rc = de.upload(end, n * 8, 0, "end rows")) ||
+        (rc = db.upload(base, n, 0, "bases")) || (rc = dos.alloc(n, "neighbour start rows")) ||
+        (rc = doe.alloc(n, "neighbour end rows")))
+        return rc;
     k_fm_neighbors<<<(n + 127) / 128, 128>>>(x->ix, n, ds, de, db, dos, doe);
-    cudaMemcpy(ostart, dos, n * 8, cudaMemcpyDeviceToHost);
-    cudaError_t e = cudaMemcpy(oend, doe, n * 8, cudaMemcpyDeviceToHost);
-    cudaFree(ds); cudaFree(de); cudaFree(dos); cudaFree(doe); cudaFree(db);
-    if (e != cudaSuccess) return fail(UNC_E_CUDA, cudaGetErrorString(e));
+    CUDA_TRY(cudaMemcpy(ostart, dos, n * 8, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(oend, doe, n * 8, cudaMemcpyDeviceToHost));
     return UNC_OK;
 }
 
 int unc_fm_sa(const unc_index *x, uint32_t n, const uint64_t *rows, uint64_t *out) {
     if (!x || !n) return fail(UNC_E_ARG, "null argument");
     CUDA_TRY(cudaSetDevice(x->device));
-    u64 *dr, *dout;
-    CUDA_TRY(cudaMalloc(&dr, n * 8)); CUDA_TRY(cudaMalloc(&dout, n * 8));
-    cudaMemcpy(dr, rows, n * 8, cudaMemcpyHostToDevice);
+    DevMem<u64> dr, dout;
+    int rc;
+    if ((rc = dr.upload(rows, n * 8, 0, "rows")) || (rc = dout.alloc(n, "suffix array values"))) return rc;
     k_fm_sa<<<(n + 127) / 128, 128>>>(x->ix, n, dr, dout);
-    cudaError_t e = cudaMemcpy(out, dout, n * 8, cudaMemcpyDeviceToHost);
-    cudaFree(dr); cudaFree(dout);
-    if (e != cudaSuccess) return fail(UNC_E_CUDA, cudaGetErrorString(e));
+    CUDA_TRY(cudaMemcpy(out, dout, n * 8, cudaMemcpyDeviceToHost));
     return UNC_OK;
 }
 
@@ -877,6 +942,14 @@ int unc_pool_k1_stats(const unc_pool *P, uint32_t out[4]) {
 int unc_pool_last_timing(const unc_pool *P, unc_timing *t) {
     if (!P || !t) return fail(UNC_E_ARG, "null argument");
     *t = P->last;
+    return UNC_OK;
+}
+
+int unc_debug_held(uint64_t *device_bytes, uint64_t *pinned_bytes, uint32_t *handles) {
+    if (!device_bytes || !pinned_bytes || !handles) return fail(UNC_E_ARG, "null argument");
+    *device_bytes = g_held_device;
+    *pinned_bytes = g_held_pinned;
+    *handles = g_held_handles;
     return UNC_OK;
 }
 
