@@ -284,6 +284,43 @@ float unc_stream_last_step_ms(const unc_stream *st);
 int unc_stream_channel_norm(const unc_stream *st, uint32_t channel, double *mean, double *varsum, uint32_t *n, uint32_t *wr);
 void unc_stream_free(unc_stream *st);
 
+/* ---- offline replay of whole reads (`uncalled_map_ord`) on a stream ---------------------------------
+ *   unc_stream_replay   MapPoolOrd::update -> RealtimePool::try_add_chunk / is_read_finished / update, until every
+ *                       read of the window is finished      src/map_pool_ord.cpp:61-121, src/realtime_pool.cpp:108-139
+ * A window is a list of whole reads of any subset of the stream's channels; the reads of one channel are listed in the
+ * order they follow each other on it (reads of different channels may interleave).  Each channel steps through its
+ * reads on the device exactly as the lockstep loop of MapPoolOrd would: one step hands the front read its next chunk
+ * (chunk i = samples [i*max_chunk_len, ...), the last one possibly partial), or, past the end of the signal, the empty
+ * chunk that means "no more signal"; a read that finishes is replaced by the next one at the following step.  No host
+ * round trip happens between the chunks of a channel.  The records depend only on the channel's earlier reads (the
+ * reference accepts a channel's next chunk only once the previous one is mapped, and MAP_ORD has no timeouts), so a
+ * run cut into several windows gives the records of one window.  The stream's chunk timeout does not apply.
+ * Every descriptor is validated before any channel's state changes.  out[] receives one entry per read, in completion
+ * order: by step, then kind, then channel, which is the order a lockstep loop over unc_stream_step returns them in.
+ * UNC_E_OVERFLOW: a channel overflowed its seed-cluster workspace (that read's rec.status != 0; out[] is complete).
+ * MapPoolOrd's min_active_reads is applied by the caller on the steps (api.MapPoolOrd, DESIGN.md section 4). */
+typedef struct {
+    uint32_t channel;     /* 0-based channel index */
+    uint32_t number;      /* read number (ReadBuffer::number_), reported back */
+    uint64_t offset;      /* in samples from `samples` */
+    uint64_t n_samples;   /* > 0 */
+    uint32_t dtype;       /* UNC_DTYPE_F32 / UNC_DTYPE_I16, one per window */
+    float cal_range, cal_offset, cal_digit;
+} unc_replay_read;
+
+typedef struct {
+    uint32_t read;        /* index of the read in the window */
+    uint32_t number;      /* its read number */
+    uint64_t step;        /* the channel's replay step that finished it (counted from 0 over all of the stream's
+                             replays; a read that finishes at step s is followed by the next one at s + 1) */
+    uint32_t kind;        /* 0: finished by the "no more signal" chunk, 1: by a chunk with samples */
+    uint32_t pad_;
+    unc_stream_result res;   /* as unc_stream_step reports the read's last step */
+} unc_replay_result;
+
+int unc_stream_replay(unc_stream *st, const unc_replay_read *reads, uint32_t n, const void *samples,
+                      unc_replay_result *out);
+
 /* ---- `uncalled index` after the BWA build ----------------------------------------------------------
  *   unc_self_align      self_align(bwa_prefix, sample_dist) -> vector<vector<u64>>
  *                                                      src/self_align_ref.cpp:34-91 (Python: src/pybinder.cpp:59,

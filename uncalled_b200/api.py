@@ -57,6 +57,8 @@ class Conf:
         "port": (8000, "MinKNOW port"),
         "duration": (72.0, "Duration to map real-time run in hours"),
         "max_active_reads": (512, "Maximum number of reads being mapped at once"),
+        "min_active_reads": (0, "map-ord: stop once fewer channels than this have a read in progress after a step "
+                                "(0: never)"),
         "device": (0, "CUDA device of this process (one process per GPU)"),
         "batch_reads": (4096, "Reads per GPU batch"),
         "exact_ties": (0, "1: children that compare equal in the per-event sort are ordered exactly as the reference's "
@@ -593,3 +595,286 @@ class RealtimePool:
             self._stopped = True
             if hasattr(self.backend, "close"):
                 self.backend.close()
+
+
+class _OrdRead:
+    __slots__ = ("id", "channel", "number", "start", "key", "n", "signal", "cal", "dtype", "src")
+
+    def __init__(self, rid, channel, number, start, key, n, signal, cal, dtype, src):
+        self.id, self.channel, self.number, self.start, self.key = rid, channel, number, start, key
+        self.n, self.signal, self.cal, self.dtype, self.src = n, signal, cal, dtype, src
+
+
+class MapPoolOrd:
+    """reference src/map_pool_ord.hpp:33-62 (`uncalled_map_ord`): MapPoolOrd(conf), add_fast5, add_read(read_id),
+    load_fast5s, update() -> [Paf], running(), stop().  Every channel's reads are replayed in the order they were
+    sequenced, through the streaming mapper with its long-lived per-channel state, as UNCALLED would have mapped them in
+    real time.  The replay runs on the device (unc_stream_replay): the reads go over in windows of at most
+    `window_samples` samples, each channel steps through its chunks without a host round trip, and the next window's
+    signals are decoded while the device replays the current one.  The records do not depend on the window size.
+
+    Observable differences from the reference (DESIGN.md section 4):
+      * reads of one channel with equal start samples keep the order of their files and of their position in the file
+        (the reference's pdqsort leaves that order unspecified);
+      * a channel number above conf.num_channels raises ValueError in load_fast5s (out of bounds in the reference);
+      * a read without samples is skipped (the reference never finishes it and runs forever);
+      * min_active_reads counts, after each step of the lockstep loop, the channels with a read in progress (the
+        reference counts at thread-timing-dependent moments);
+      * all reads of a run share one sample type (int16 from fast5 files)."""
+
+    def __init__(self, conf, backend=None, index=None, window_samples=1 << 28):
+        """`backend`/`index` (tests): an object with replay(reads, n, flat, out) standing in for the StreamMapper, and an
+        index with .seqs.  The index is loaded at the first update(), so that input errors are found first."""
+        self.conf = conf
+        self.chunk_len = int(np.float32(conf.chunk_time) * np.float32(conf.sample_rate)) & 0xFFFF   # u16 chunk_len()
+        self.backend, self.index = backend, index
+        self.window_samples = int(window_samples)
+        self._files, self._ids = [], None
+        if conf.fast5_list:                                   # Fast5Reader::load_fast5_list
+            self._files = [l.rstrip("\n") for l in open(conf.fast5_list) if l.strip()]
+        if conf.read_list:
+            self._ids = set(l.strip() for l in open(conf.read_list) if l.strip())
+        self._mem = []                                        # queue_read
+        self._channels = None                                 # per channel: its reads in replay order
+        self._open = {}
+        self._future, self._executor = None, None
+        self._stopped = False
+        n = conf.num_channels
+        self._next_start = [0] * n                            # the step at which the channel's next read starts
+        self._starts, self._fins = [], []                     # every replayed read's first and last step
+        self._held = []                                       # results after the step up to which activity is known
+        self._known = -1
+
+    # -- input ---------------------------------------------------------------------------
+    def add_fast5(self, fname):
+        self._files.append(fname)
+
+    def add_read(self, read_id):
+        """Fast5Reader::add_read: only the reads named so are mapped (map_pool_ord.cpp:44)."""
+        if self._ids is None:
+            self._ids = set()
+        self._ids.add(read_id)
+
+    def queue_read(self, read_id, signal, channel, number=0, start_sample=0, calibration=None):
+        """Queue one in-memory read (as MapPool.add_read): float32 pA, or int16 DAC values with calibration=(range,
+        offset, digitisation).  `channel` is 1-based.  Reads queued so come after those of the fast5 files when start
+        samples are equal."""
+        sig = np.asarray(signal)
+        if calibration is None:
+            sig, dtype, cal = np.ascontiguousarray(sig, np.float32), 0, (1.0, 0.0, 1.0)
+        else:
+            if sig.dtype != np.int16:
+                raise TypeError("calibration given: the signal must be int16 DAC values")
+            sig, dtype, cal = np.ascontiguousarray(sig), 1, tuple(float(np.float32(x)) for x in calibration)
+        self._mem.append((read_id, sig, int(channel), int(number), int(start_sample), dtype, cal))
+
+    def _max_len(self):
+        return int(self.conf.max_chunks) * self.chunk_len      # ReadBuffer keeps at most max_chunks chunks
+
+    def load_fast5s(self):
+        """MapPoolOrd::load_fast5s (map_pool_ord.cpp:48-59): every read's header is read up front (read list and
+        max_reads applied as Fast5Reader does), reads are grouped by channel and each channel is sorted by start sample,
+        ties by file order and position in the file.  Signals are decoded window by window.  Raises ValueError for a
+        channel outside 1..num_channels."""
+        from .fast5 import Fast5File
+        n_ch, cap = self.conf.num_channels, self.conf.max_reads
+        reads, k = [], 0
+        for fi, path in enumerate(self._files):
+            if cap and k >= cap:
+                break
+            with Fast5File(path) as f:
+                for i in range(f.n_reads):
+                    if cap and k >= cap:
+                        break
+                    info = f.info(i)
+                    if self._ids is not None and info.read_id not in self._ids:
+                        continue
+                    k += 1
+                    n = min(info.n_samples, self._max_len())
+                    if n:
+                        reads.append(_OrdRead(info.read_id, int(info.channel), int(info.number), int(info.start_sample),
+                                              (int(info.start_sample) % (1 << 64), fi, i), n, None, None, 1, (path, i)))
+        for j, (rid, sig, ch, nm, st, dtype, cal) in enumerate(self._mem):
+            if (self._ids is not None and rid not in self._ids) or (cap and k >= cap):
+                continue
+            k += 1
+            sig = sig[:self._max_len()]
+            if len(sig):
+                reads.append(_OrdRead(rid, ch, nm, st, (st % (1 << 64), len(self._files), j), len(sig), sig, cal, dtype,
+                                      None))
+        bad = [r for r in reads if not 1 <= r.channel <= n_ch]
+        if bad:
+            raise ValueError("read %s is on channel %d, outside 1..%d (--num-channels)" % (bad[0].id, bad[0].channel, n_ch))
+        if len(set(r.dtype for r in reads)) > 1:
+            raise ValueError("the reads mix float32 and int16 signals")
+        self._channels = [[] for _ in range(n_ch)]
+        for r in reads:
+            self._channels[r.channel - 1].append(r)
+        for q in self._channels:
+            q.sort(key=lambda r: r.key)
+        self._left = [len(q) for q in self._channels]
+        self.n_loaded = len(reads)
+        return len(reads)
+
+    def _fetch(self, reads):
+        """Decodes the signals of a window's fast5 reads (their sample counts after the max_chunks cut)."""
+        from .fast5 import Fast5File
+        for r in reads:
+            if r.signal is None:
+                path, i = r.src
+                f = self._open.get(path)
+                if f is None:
+                    f = self._open[path] = Fast5File(path)
+                rd = f.load(i, 1, max_samples_per_read=self._max_len(), threads=self.conf.threads)[0]
+                r.signal, r.cal, r.n = rd.signal, rd.calibration, len(rd.signal)
+        return reads
+
+    def _take_window(self):
+        """The next reads of the channels, one per channel per round, while they fit in window_samples (at least one)."""
+        win, total = [], 0
+        while True:
+            took = False
+            for q in self._channels:
+                if q and (not win or total + q[0].n <= self.window_samples):
+                    win.append(q.pop(0))
+                    total += win[-1].n
+                    took = True
+            if not took:
+                return win
+
+    # -- output --------------------------------------------------------------------------
+    def _ensure_backend(self):
+        if self.backend is not None:
+            return
+        from .stream import StreamMapper
+        if not self.conf.bwa_prefix:
+            raise RuntimeError("Conf.bwa_prefix is not set")
+        self.index = Index(self.conf.bwa_prefix, preset=self.conf.idx_preset, device=self.conf.device,
+                           model_table=self.conf.model_path or None)
+        p = N.default_params()
+        p.max_events, p.max_paths, p.seed_len = self.conf.max_events, self.conf.max_paths, self.conf.seed_len
+        p.bp_per_sec, p.sample_rate = self.conf.bp_per_sec, self.conf.sample_rate
+        self.backend = StreamMapper(self.index, self.conf.num_channels, self.chunk_len, max_chunks=self.conf.max_chunks,
+                                    params=p)
+        if self.conf.exact_ties:
+            self.backend.set_tie_order(1)
+
+    def _prefetch(self):
+        win = self._take_window()
+        if not win:
+            return None
+        if any(r.signal is None for r in win):
+            if self._executor is None:
+                from concurrent.futures import ThreadPoolExecutor
+                self._executor = ThreadPoolExecutor(max_workers=1)
+            return self._executor.submit(self._fetch, win)
+        return _Done(win)
+
+    def _replay(self, win):
+        from . import stream as S
+        reads = (S.ReplayRead * len(win))()
+        off = 0
+        for d, r in zip(reads, win):
+            d.channel, d.number, d.offset, d.n_samples, d.dtype = r.channel - 1, r.number & 0xFFFFFFFF, off, r.n, r.dtype
+            d.cal_range, d.cal_offset, d.cal_digit = r.cal
+            off += r.n
+        flat = np.concatenate([r.signal for r in win])
+        out = (S.ReplayResult * len(win))()
+        self.backend.replay(reads, len(win), flat, out)
+        seqs = self.index.seqs if self.index is not None else []
+        ret = []
+        for o in out:
+            r = win[o.read]
+            if int(o.res.rec.status) != 0:               # the channel's device workspace overflowed: never silent
+                sys.stderr.write("Warning: read %s (channel %d) overflowed its device workspace (status %d); reported "
+                                 "unmapped\n" % (r.id, r.channel, int(o.res.rec.status)))
+            p = _paf_from_rec(seqs, o.res.rec, r.id, r.channel, r.start)
+            if o.res.ended:
+                p._ended = True                            # Paf::set_ended
+            p.chunks, p.rec = int(o.res.chunks), N.PafRec.from_buffer_copy(bytes(o.res.rec))   # chunks used, raw record
+            ch = r.channel - 1
+            self._starts.append(self._next_start[ch])
+            self._fins.append(int(o.step))
+            self._next_start[ch] = int(o.step) + 1
+            self._left[ch] -= 1
+            ret.append((int(o.step), p))
+            r.signal = None
+        return ret
+
+    def _gate(self, results):
+        """min_active_reads: the run stops after the first step t at which fewer channels than that have a read in progress
+        (started at or before t, finished after t).  Results are held back until activity is known up to their step."""
+        m = int(self.conf.min_active_reads)
+        if m <= 0:
+            return [p for _, p in results]
+        self._held += results
+        pending = [self._next_start[c] - 1 for c, k in enumerate(self._left) if k]
+        horizon = min(pending) if pending else max(self._fins, default=0)
+        st, fi = np.sort(np.array(self._starts, np.int64)), np.sort(np.array(self._fins, np.int64))
+        cand = np.unique(np.concatenate([[0], fi]))
+        cand = cand[(cand > self._known) & (cand <= horizon)]
+        active = np.searchsorted(st, cand, side="right") - np.searchsorted(fi, cand, side="right")
+        low = np.flatnonzero(active < m)
+        stop = int(cand[low[0]]) if len(low) else None
+        upto = stop if stop is not None else horizon
+        out = [p for s, p in self._held if s <= upto]
+        self._held = [(s, p) for s, p in self._held if s > upto]
+        self._known = max(self._known, upto)
+        if stop is not None:
+            self._stop_all()
+        return out
+
+    def update(self):
+        """Replays the next window on the device and returns its reads' Paf records, in completion order.  Each Paf also
+        carries `chunks` (chunks the decision took) and `rec` (the device record, unc_paf_rec)."""
+        if self._stopped:
+            return []
+        if self._channels is None:
+            self.load_fast5s()
+        self._ensure_backend()
+        cur = self._future if self._future is not None else self._prefetch()
+        self._future = None
+        if cur is None:
+            self._stopped = True
+            return self._gate([]) if self._held else []
+        win = cur.result()
+        self._future = self._prefetch()                   # decoded while the device replays this window
+        return self._gate(self._replay(win))
+
+    def running(self):
+        return not self._stopped and (self._channels is None or self._future is not None or bool(self._held) or
+                                      any(self._channels))
+
+    def _stop_all(self):
+        self._stopped = True
+        for q in self._channels or []:
+            q.clear()
+        self._left = [0] * len(self._left)
+        self._held = []
+
+    def stop(self):
+        self._stopped = True
+        if self._future is not None:
+            try:
+                self._future.result()
+            except Exception:
+                pass
+            self._future = None
+        if self._executor is not None:
+            self._executor.shutdown(wait=True)
+            self._executor = None
+        for f in self._open.values():
+            f.close()
+        self._open = {}
+        if self.backend is not None and hasattr(self.backend, "close"):
+            self.backend.close()
+
+
+class _Done:
+    """A window whose signals are already in memory (the Future interface the prefetch uses)."""
+
+    def __init__(self, v):
+        self.v = v
+
+    def result(self):
+        return self.v

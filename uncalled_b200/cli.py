@@ -52,6 +52,25 @@ def get_parser(conf):
     p.add_argument("--ordered", action="store_const", const=1, default=conf.ordered, help=type(conf).ordered.__doc__)
     p.add_argument("--exact-ties", action="store_const", const=1, default=conf.exact_ties, help=type(conf).exact_ties.__doc__)
 
+    p = sp.add_parser("map-ord", help="Map fast5 files as UNCALLED would have in real time: every channel's reads replayed "
+                      "in the order they were sequenced, chunk by chunk, through the streaming mapper", formatter_class=fmt)
+    p.add_argument("bwa_prefix", type=str, help="BWA prefix to mapping to. Must be processed by \"uncalled index\".")
+    p.add_argument("-p", "--idx-preset", type=str, default=conf.idx_preset, help="Mapping mode")
+    p.add_argument("fast5s", nargs="+", type=str, help="Reads to map. Can be a directory which will be recursively searched "
+                   "for all files with the \".fast5\" extension, a text file containing one fast5 filename per line, or a "
+                   "comma-separated list of fast5 file names.")
+    p.add_argument("-r", "--recursive", action="store_true")
+    p.add_argument("-l", "--read-list", type=str, default=None, help=type(conf).read_list.__doc__)
+    p.add_argument("-n", "--max-reads", type=int, default=None, help=type(conf).max_reads.__doc__)
+    p.add_argument("-t", "--threads", type=int, default=conf.threads, help="Number of host threads (fast5 decoding; the mapping runs on the GPU)")
+    p.add_argument("--num-channels", type=int, default=conf.num_channels, help="Number of channels used in sequencing.")
+    p.add_argument("-e", "--max-events", type=int, default=conf.max_events, help="Will give up on a read after this many events have been processed")
+    p.add_argument("-c", "--max-chunks", type=int, default=conf.max_chunks, help="Will give up on a read after this many chunks have been processed.")
+    p.add_argument("--chunk-time", type=float, default=1, required=False, help="Length of chunks in seconds")
+    p.add_argument("--min-active-reads", type=int, default=conf.min_active_reads, help=type(conf).min_active_reads.__doc__)
+    p.add_argument("--exact-ties", action="store_const", const=1, default=conf.exact_ties, help=type(conf).exact_ties.__doc__)
+    p.add_argument("--device", type=int, default=conf.device, help="CUDA device")
+
     p = sp.add_parser("sim", help="Simulate real-time targeted sequencing (read until) from a control run and an "
                       "UNCALLED run", formatter_class=fmt)
     p.add_argument("bwa_prefix", type=str, help="BWA prefix to mapping to. Must be processed by \"uncalled index\".")
@@ -199,6 +218,38 @@ def map_cmd(conf, args, out=None):
     mapper.stop()
 
 
+def map_ord_cmd(conf, args, out=None, backend=None, index=None):
+    """uncalled_map_ord (reference src/uncalled_map_ord.cpp): every read is loaded up front, then the channels are replayed
+    on the device; PAF goes to `out` (stdout), progress to stderr.  A missing index file or read list, or a read on a
+    channel above --num-channels, ends the command with status 1 before the GPU is touched."""
+    from .api import MapPoolOrd
+    if backend is None:
+        assert_exists(conf.bwa_prefix + ".bwt")
+        assert_exists(conf.bwa_prefix + ".uncl")
+    if len(conf.read_list) > 0:
+        assert_exists(conf.read_list)
+    pool = MapPoolOrd(conf, backend=backend, index=index)
+    for fast5 in load_fast5s(args.fast5s, args.recursive):
+        if fast5 is not None:
+            pool.add_fast5(fast5)
+    sys.stderr.write("Loading fast5s\n")
+    try:
+        pool.load_fast5s()
+    except ValueError as e:
+        sys.stderr.write("Error: %s\n" % e)
+        sys.exit(1)
+    sys.stderr.write("Mapping\n")
+    sys.stderr.flush()
+    try:
+        while pool.running():
+            for p in pool.update():
+                p.print_paf(out)
+    except KeyboardInterrupt:
+        pass
+    sys.stderr.write("Finishing\n")
+    pool.stop()
+
+
 def sim_cmd(conf, args, out=None):
     """scripts/uncalled:169-300 with `sim`: the pattern and the control reads are loaded, then the decision loop runs
     until every simulated channel has run out.  Bad input ends the command with status 1 before the GPU is touched."""
@@ -295,6 +346,8 @@ def main(argv=None):
         index_cmd(args)
     elif args.subcmd == "map":
         map_cmd(conf, args)
+    elif args.subcmd == "map-ord":
+        map_ord_cmd(conf, args)
     elif args.subcmd == "sim":
         sim_cmd(conf, args)
     elif args.subcmd == "mask-internal":

@@ -2,12 +2,19 @@
 // Mapper::new_read(Chunk&) / add_chunk / request_reset applies to an arriving chunk, and what
 // Mapper::map_chunk concludes once the chunk's events are mapped (reference src/mapper.cpp:210-218,
 // 281-299, 381-431; src/read_buffer.cpp:249-296; src/realtime_pool.cpp:108-139).
-// Pure C++ (shared by the CUDA library and by the CPU emulator harness of the tests).
+// Pure C++, __host__ __device__ under nvcc: one copy for unc_stream_step (host), the device replay of
+// unc_stream_replay (unc_replay.cuh, thread 0 of a CTA) and the CPU emulator harness of the tests.
 #pragma once
 #include <stdint.h>
 #include <string.h>
 
 #include "../../include/unc_b200.h"
+
+#ifdef __CUDACC__
+#define UNC_HD __host__ __device__
+#else
+#define UNC_HD
+#endif
 
 struct HostChan {
     int state = UNC_STREAM_INACTIVE;
@@ -17,11 +24,11 @@ struct HostChan {
     int max_events_hit = 0;      // event_i_ reached max_events with the chunk fully mapped: map_chunk has not looked yet
     unc_paf_rec rec;
     uint64_t n_children = 0, n_sources = 0, n_occ_blocks = 0, n_sa_steps = 0, n_seeds = 0;
-    HostChan() { memset(&rec, 0, sizeof(rec)); rec.rid = -1; }
+    UNC_HD HostChan() { memset(&rec, 0, sizeof(rec)); rec.rid = -1; }
 };
 
 // Returns true when the chunk must be processed on the device.
-static inline bool stream_admit(HostChan &h, const unc_chunk_desc &c, uint32_t max_chunks) {
+static UNC_HD inline bool stream_admit(HostChan &h, const unc_chunk_desc &c, uint32_t max_chunks) {
     if (c.new_read) {                                   // Mapper::new_read(Chunk&) -> ReadBuffer(Chunk&)
         h = HostChan();
         h.state = UNC_STREAM_MAPPING; h.chunk_count = 1; h.raw_len = c.n_samples;
@@ -42,7 +49,7 @@ static inline bool stream_admit(HostChan &h, const unc_chunk_desc &c, uint32_t m
 }
 
 // After the device mapped the chunk's events: `r` is the mapper's record of this step.
-static inline void stream_settle(HostChan &h, const unc_paf_rec &r, uint32_t total_events, uint32_t max_events,
+static UNC_HD inline void stream_settle(HostChan &h, const unc_paf_rec &r, uint32_t total_events, uint32_t max_events,
                                  uint32_t max_chunks) {
     h.n_children += r.n_children; h.n_sources += r.n_sources; h.n_occ_blocks += r.n_occ_blocks;
     h.n_sa_steps += r.n_sa_steps; h.n_seeds += r.n_seeds;
@@ -64,7 +71,7 @@ static inline void stream_settle(HostChan &h, const unc_paf_rec &r, uint32_t tot
     else if (chunk_events == 0 && h.chunk_count >= max_chunks) h.state = UNC_STREAM_FAILURE;
 }
 
-static inline void stream_result(const HostChan &h, float bp_per_samp, unc_stream_result *o) {
+static UNC_HD inline void stream_result(const HostChan &h, float bp_per_samp, unc_stream_result *o) {
     o->state = h.state; o->ended = h.ended; o->chunks = h.chunk_count; o->pad_ = 0;
     o->rec = h.rec;
     o->rec.n_children = h.n_children; o->rec.n_sources = h.n_sources; o->rec.n_occ_blocks = h.n_occ_blocks;

@@ -15,11 +15,12 @@ class Fast5Error(RuntimeError):
 
 
 class Fast5Read:
-    __slots__ = ("read_id", "number", "start_sample", "channel", "calibration", "signal")
+    __slots__ = ("read_id", "number", "start_sample", "channel", "calibration", "signal", "n_samples")
 
     def __init__(self, info, signal):
         self.read_id = (info.read_id or b"").decode("utf-8", "replace")
         self.number, self.start_sample, self.channel = info.number, info.start_sample, info.channel
+        self.n_samples = int(info.n_samples)         # the signal's length in the file
         self.calibration = (info.cal_range, info.cal_offset, info.cal_digitisation)   # MapPool.add_read order
         self.signal = signal
 

@@ -26,6 +26,18 @@ class StreamResult(C.Structure):
                 ("rec", N.PafRec)]
 
 
+class ReplayRead(C.Structure):
+    """unc_replay_read"""
+    _fields_ = [("channel", C.c_uint32), ("number", C.c_uint32), ("offset", C.c_uint64), ("n_samples", C.c_uint64),
+                ("dtype", C.c_uint32), ("cal_range", C.c_float), ("cal_offset", C.c_float), ("cal_digit", C.c_float)]
+
+
+class ReplayResult(C.Structure):
+    """unc_replay_result"""
+    _fields_ = [("read", C.c_uint32), ("number", C.c_uint32), ("step", C.c_uint64), ("kind", C.c_uint32),
+                ("pad_", C.c_uint32), ("res", StreamResult)]
+
+
 def feed_reads(step, n_channels, signals, chunk_len, max_chunks=1000000):
     """Drives `step(descs, n, flat_samples, results)` like a flow cell: read i sits on channel i % n_channels
     (reads sharing a channel follow each other); every round each active channel gets its next FULL chunk, and
@@ -112,6 +124,16 @@ class StreamMapper:
         rc = self.L.unc_stream_step(self.h, descs, n, flat.ctypes.data, res)
         if rc != 0 and rc != -7:
             N.check(rc)
+
+    def replay(self, reads, n, flat, out):
+        """unc_stream_replay: a window of whole reads (ReplayRead array) run to completion on the device; `out` (ReplayResult
+        array of n) receives them in completion order.  Returns 0 or UNC_E_OVERFLOW (-7, reported per read in
+        rec.status); other errors raise."""
+        flat = np.ascontiguousarray(flat)
+        rc = self.L.unc_stream_replay(self.h, reads, n, flat.ctypes.data, out)
+        if rc != 0 and rc != -7:
+            N.check(rc)
+        return rc
 
     def map_reads(self, signals):
         """Streams whole reads through the channels (feed_reads policy); one result per read."""
