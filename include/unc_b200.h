@@ -350,6 +350,15 @@ typedef struct { int32_t subseq; float dw, hw, vw; } unc_dtw_params;
 int unc_dtw_batch(const float *model_means_stdvs, int cost_kind, const unc_dtw_params *prm, uint32_t n_problems,
                   const float *means, const uint64_t *mean_off, const uint16_t *kmers, const uint64_t *kmer_off,
                   uint64_t *path, const uint64_t *path_off, uint64_t *path_len, float *score);
+/* unc_dtw_batch_banded: unc_dtw_batch restricted to a band of rows around the diagonal (the recurrence of
+ * src/dtw.hpp:51-120, its traceback unchanged), for subseq NONE only (else UNC_E_ARG; band = 0 is UNC_E_ARG too).  Column
+ * j of an R x C problem holds rows max(0, c - We) .. min(R-1, c + We), c = floor(j (R-1) / (C-1)) (0 when C = 1), We =
+ * max(band, ceil((R-1) / (C-1))) (R - 1 when C = 1); a predecessor outside the band scores FLT_MAX / 2, as one outside the
+ * matrix does.  Same outputs as unc_dtw_batch.  The score is never below the full sweep's and equals it whenever the full
+ * path lies in the band; band >= R gives unc_dtw_batch's results.  The workspace holds one byte per in-band cell. */
+int unc_dtw_batch_banded(const float *model_means_stdvs, int cost_kind, const unc_dtw_params *prm, uint32_t n_problems,
+                         const float *means, const uint64_t *mean_off, const uint16_t *kmers, const uint64_t *kmer_off,
+                         uint64_t *path, const uint64_t *path_off, uint64_t *path_len, float *score, uint32_t band);
 /* The device workspace of unc_dtw_batch is kept between calls and grown on demand; unc_dtw_release (also called by
  * unc_shutdown) frees it.  unc_dtw_last_kernel_ms: CUDA-event time of the last call's sweep kernel. */
 void unc_dtw_release(void);
@@ -396,6 +405,11 @@ int unc_dtw_aligner_create(const char *bwa_prefix, const char *model_table_path,
 void unc_dtw_aligner_free(unc_dtw_aligner *a);
 int unc_dtw_aligner_contig(const unc_dtw_aligner *a, const char *name, int32_t *rid, uint64_t *len);
 int unc_dtw_aligner_set_budget(unc_dtw_aligner *a, uint64_t bytes);
+/* unc_dtw_aligner_set_band: 0 (the default) aligns with the full matrix, as the reference does, and skips reads over 50 000
+ * kept means; band >= 1 aligns with unc_dtw_batch_banded's sweep at that half-width (the recurrence of src/dtw.hpp:51-120
+ * restricted to the band), where only the workspace budget limits a read's length: a query whose band alone exceeds it is
+ * skipped with UNC_DTW_ALIGN_TOO_LARGE.  unc_dtw_align_last_times then counts in-band cells. */
+int unc_dtw_aligner_set_band(unc_dtw_aligner *a, uint32_t band);
 int unc_dtw_align_batch(unc_dtw_aligner *a, uint32_t n, const unc_read_desc *reads, const void *samples,
                         const unc_dtw_query *q, int keep_paths, unc_dtw_align_result *res);
 int unc_dtw_align_path(const unc_dtw_aligner *a, uint32_t i, uint64_t *pairs, float *means, uint16_t *kmers);

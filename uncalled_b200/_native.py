@@ -89,7 +89,7 @@ EXPORTS = ["unc_strerror", "unc_last_error", "unc_device_count", "unc_init", "un
            "unc_mask_external_last_times", "unc_index_build_device", "unc_index_build_device_last_times",
            "unc_index_build_device_last_active", "unc_dtw_aligner_create", "unc_dtw_aligner_free", "unc_dtw_aligner_contig",
            "unc_dtw_aligner_set_budget", "unc_dtw_align_batch", "unc_dtw_align_path", "unc_dtw_align_last_times",
-           "unc_debug_held"]
+           "unc_debug_held", "unc_dtw_batch_banded", "unc_dtw_aligner_set_band"]
 
 
 def build(force=False, verbose=False):
@@ -97,7 +97,7 @@ def build(force=False, verbose=False):
     src_dir = os.path.join(PKG_DIR, "csrc")
     srcs = [os.path.join(src_dir, f) for f in ("unc_abi.cu", "unc_index_build.cpp", "unc_fast5.cpp")]
     deps = srcs + [os.path.join(src_dir, f) for f in
-                   ("unc_device.cuh", "unc_k2v2.cuh", "unc_dtw.cuh", "unc_dtw_host.inl", "unc_dtw_align.cuh", "unc_dtw_align_host.inl", "unc_k1.cuh", "unc_stream.cuh", "unc_stream_host.inl", "unc_stream_logic.hpp", "unc_replay.cuh", "unc_replay_host.inl", "unc_ordered_logic.hpp", "unc_pdqsort.cuh", "unc_warp.cuh",
+                   ("unc_device.cuh", "unc_k2v2.cuh", "unc_dtw.cuh", "unc_dtw_band.cuh", "unc_dtw_host.inl", "unc_dtw_align.cuh", "unc_dtw_align_host.inl", "unc_k1.cuh", "unc_stream.cuh", "unc_stream_host.inl", "unc_stream_logic.hpp", "unc_replay.cuh", "unc_replay_host.inl", "unc_ordered_logic.hpp", "unc_pdqsort.cuh", "unc_warp.cuh",
                     "unc_selfalign.cuh", "unc_selfalign_host.hpp", "unc_selfalign_host.inl",
                     "unc_mask.cuh", "unc_mask_host.hpp", "unc_mask_host.inl",
                     "unc_mask_ext.cuh", "unc_mask_ext_host.hpp", "unc_mask_ext_host.inl",
@@ -215,6 +215,7 @@ def lib():
     L.unc_dtw_aligner_free.restype = None
     L.unc_dtw_aligner_contig.argtypes = [vp, C.c_char_p, C.POINTER(C.c_int32), C.POINTER(u64)]
     L.unc_dtw_aligner_set_budget.argtypes = [vp, u64]
+    L.unc_dtw_aligner_set_band.argtypes = [vp, u32]
     L.unc_dtw_align_batch.argtypes = [vp, u32, vp, vp, vp, C.c_int, vp]
     L.unc_dtw_align_path.argtypes = [vp, u32, vp, vp, vp]
     L.unc_dtw_align_last_times.argtypes = [vp, vp, C.POINTER(u64), C.POINTER(u64)]

@@ -128,6 +128,8 @@ def get_parser(conf):
     p.add_argument("--queries", required=True, type=str, help="One query per line: rd_name rd_st rd_en rf_name rf_st "
                    "rf_en strand (samples [rd_st, rd_en) of the read, 0 0 = all of it; bases [rf_st, rf_en) of the contig)")
     p.add_argument("--path-prefix", type=str, default="", help="Also write each read's DTW path to <prefix><read_id>.txt")
+    p.add_argument("--band", type=int, default=0, help="Align within this many rows (k-mers) of the diagonal instead of "
+                   "the whole matrix (0: the whole matrix, and reads over 50 000 kept means are skipped)")
     p.add_argument("-r", "--recursive", action="store_true", help="Recursively search 'fast5s' for fast5 files")
     p.add_argument("--device", type=int, default=0, help="CUDA device")
 
@@ -276,7 +278,10 @@ def dtw_cmd(args, out=None):
     for ext in (".pac", ".ann"):
         assert_exists(args.bwa_prefix + ext)
     assert_exists(args.queries)
-    aligner = DtwAligner(args.bwa_prefix)
+    if not 0 <= args.band < 1 << 32:
+        sys.stderr.write("Error: --band must be 0 (the whole matrix) or a half-width below 2^32\n")
+        sys.exit(1)
+    aligner = DtwAligner(args.bwa_prefix, band=args.band)
     try:
         queries = load_queries(args.queries, aligner)
     except QueryError as e:

@@ -44,12 +44,17 @@ def model_table():
     return _model
 
 
-def dtw_batch(problems, prms, cost="r94p", model=None):
+def dtw_batch(problems, prms, cost="r94p", model=None, band=0):
     """problems: sequence of (means, kmers).  Returns a list of (path, score): path = uint64 array [n, 2] of (column =
-    event index, row = k-mer index) pairs from the end of the alignment back to its start, as `get_path()` gives them."""
+    event index, row = k-mer index) pairs from the end of the alignment back to its start, as `get_path()` gives them.
+    band = 0 fills the whole matrix; band = W >= 1 only the rows within W (widened to the diagonal's slope) of each column's
+    point on the diagonal (`unc_dtw_batch_banded`, global alignment only): the score is never below the full one and equals
+    it when the full path stays in the band."""
     L = N.lib()
-    L.unc_dtw_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(DTWParams), C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
-                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    args = [C.c_void_p, C.c_int, C.POINTER(DTWParams), C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+            C.c_void_p, C.c_void_p, C.c_void_p]
+    L.unc_dtw_batch.argtypes = args
+    L.unc_dtw_batch_banded.argtypes = args + [C.c_uint32]
     n = len(problems)
     if n == 0:
         return []
@@ -67,8 +72,11 @@ def dtw_batch(problems, prms, cost="r94p", model=None):
     score = np.zeros(n, np.float32)
     tab = np.ascontiguousarray(model if model is not None else model_table(), dtype=np.float32)
     kind = {"r94p": 0, "r94d": 1}[cost]
-    N.check(L.unc_dtw_batch(tab.ctypes.data, kind, C.byref(prms), n, am.ctypes.data, moff.ctypes.data, ak.ctypes.data, koff.ctypes.data,
-                            path.ctypes.data, poff.ctypes.data, plen.ctypes.data, score.ctypes.data))
+    a = (tab.ctypes.data, kind, C.byref(prms), n, am.ctypes.data, moff.ctypes.data, ak.ctypes.data, koff.ctypes.data,
+         path.ctypes.data, poff.ctypes.data, plen.ctypes.data, score.ctypes.data)
+    if not 0 <= band < 1 << 32:
+        raise ValueError("band must be 0 (the full matrix) or a half-width from 1 to 2^32 - 1")
+    N.check(L.unc_dtw_batch_banded(*a, int(band)) if band else L.unc_dtw_batch(*a))
     return [(path[int(poff[i]):int(poff[i]) + int(plen[i])].copy(), float(score[i])) for i in range(n)]
 
 
@@ -140,13 +148,16 @@ class Alignment:
 class DtwAligner:
     """The reference's dtw_test driver (src/dtw_test.cpp:94-175) on the GPU: reads aligned by DTWr94d to their reference
     spans, after event detection, the EventProfiler mask and normalisation to the span's model levels.  Only the .pac and
-    .ann of `bwa_prefix` are read.  `budget`: bytes of the DTW sweep's workspace (0 = the free device memory)."""
+    .ann of `bwa_prefix` are read.  `budget`: bytes of the DTW sweep's workspace (0 = the free device memory).  `band`: 0
+    aligns with the full matrix and skips reads over 50 000 kept means, as the reference does; W >= 1 aligns with the banded
+    sweep of half-width W (see `dtw_batch`), where only the budget limits a read's length."""
 
-    def __init__(self, bwa_prefix, budget=0):
+    def __init__(self, bwa_prefix, budget=0, band=0):
         self._L = N.lib()
         self._h = C.c_void_p()
         N.check(self._L.unc_dtw_aligner_create(os.fsencode(bwa_prefix), os.fsencode(N.MODEL_TABLE), C.byref(self._h)))
         self.set_budget(budget)
+        self.set_band(band)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -157,6 +168,12 @@ class DtwAligner:
 
     def set_budget(self, nbytes):
         N.check(self._L.unc_dtw_aligner_set_budget(self._h, int(nbytes)))
+
+    def set_band(self, band):
+        """0: the full matrix; W >= 1: the banded sweep of half-width W"""
+        if not 0 <= band < 1 << 32:
+            raise ValueError("band must be 0 (the full matrix) or a half-width from 1 to 2^32 - 1")
+        N.check(self._L.unc_dtw_aligner_set_band(self._h, int(band)))
 
     def contig(self, name):
         """(rid, length) of a contig of the .ann, or None"""
@@ -216,7 +233,7 @@ class DtwAligner:
 
     def last_times(self):
         """CUDA-event times of the last batch in ms: h2d, events, mask, kmers, target, norm, sweep, total; then the
-        number of sweep launches and of matrix cells."""
+        number of sweep launches and of matrix cells (in-band cells with a band)."""
         ms = np.zeros(8, np.float32)
         la, ce = C.c_uint64(), C.c_uint64()
         N.check(self._L.unc_dtw_align_last_times(self._h, ms.ctypes.data, C.byref(la), C.byref(ce)))
