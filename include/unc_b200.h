@@ -28,6 +28,8 @@
  *   unc_events_batch    EventDetector::get_means + Normalizer::set_signal/pop
  *                                                      src/event_detector.cpp:133-145,
  *                                                      src/normalizer.cpp:31-44,114-129
+ *   unc_events_*        EventDetector::get_events, EventProfiler::get_full_mask, PoreModel::match_prob
+ *                       (the `events` command; see the section below)
  *   unc_pool_free       MapPool::stop                  src/map_pool.cpp:71-82
  */
 #ifndef UNC_B200_H
@@ -456,6 +458,71 @@ int unc_mask_external(const char *full_fasta, const char *target_fasta, uint32_t
                       uint64_t *n_selected, uint64_t *n_masked_bp);
 float unc_mask_external_last_kernel_ms(void);
 void unc_mask_external_last_times(float ms[4], uint64_t *h2d_bytes);
+
+/* ---- per-event view of the signal front end (`events`) -------------------------------------------------------
+ *   unc_events_create     EventDetector(Params) + EventProfiler() + PoreModel loaded from a table: no FM index is needed
+ *                         src/event_detector.cpp:17-38, src/event_profiler.cpp:3-9, src/pore_model.hpp:48-103
+ *   unc_events_run        for every read, over its whole signal (no max_events cap):
+ *                         EventDetector::get_events with create_event   src/event_detector.cpp:83-127,296-319
+ *                         (mean, stdv, start, length of each event passing min_mean / max_mean, :104-108)
+ *                         Normalizer::set_signal + at over the event means towards the model's mean and stdv, the
+ *                         offline normaliser of Mapper::map_read        src/normalizer.cpp:31-44,114-118, src/mapper.cpp:193
+ *                         EventProfiler::add_event / anno_event / get_full_mask   src/event_profiler.hpp:71-151
+ *                         (the DEBUG_EVENTS columns win_mean, win_stdv, win_mask of src/mapper.cpp:894-905,968-989)
+ *   unc_events_fetch      the events of the last run, reads in order
+ *   unc_events_annotate   the normaliser and EventProfiler::get_full_mask over event means the caller supplies
+ *   unc_match_probs_batch PoreModel::match_prob for many means at once  src/pore_model.hpp:163-165
+ * Reads are described as for unc_map_batch (f32 pA, or i16 DAC calibrated on the device, one dtype per call).  win_mean
+ * and win_stdv of an event are those of the add_event call after which it is next_evt_ (what anno_event() returns for
+ * it); the last events of a read never get there and have NaN in both, and the tail loop of get_full_mask's mask.  The
+ * scale and shift are the ones Normalizer::at computes (double division rounded to float), as the mapper applies them;
+ * a read without events has scale = shift = 0.  Window lengths 3 / 6 and the profiler's 25-event window are fixed in
+ * the device code (UNC_E_ARG otherwise).  Device memory: 32 bytes per sample of the largest run, plus the samples. */
+typedef struct {
+    uint32_t window_length1, window_length2;    /* 3, 6: fixed */
+    float threshold1, threshold2, peak_height;  /* 1.4, 9.0, 0.2 */
+    float min_mean, max_mean;                   /* 0, 400 */
+    uint32_t win_len;                           /* EventProfiler::Params: 25, fixed */
+    float win_stdv_min;                         /* 5 */
+} unc_event_params;
+
+typedef struct {          /* one event: Event (src/event_detector.hpp:19-24) and its annotations */
+    uint32_t start;
+    float length;         /* Event::length is an integer number of samples; exact in a float below 2^24 */
+    float mean, stdv;
+    float norm_mean;      /* scale * mean + shift */
+    float win_mean, win_stdv;
+    uint32_t win_mask;    /* 1: kept (get_full_mask true), 0: masked as a stall */
+} unc_event_full;
+
+typedef struct {
+    uint32_t n_events;    /* events that passed the min_mean / max_mean filter */
+    float mean_event_len; /* EventDetector::mean_event_len over every event, filtered or not (NaN without any) */
+    float norm_scale, norm_shift;
+} unc_event_read;
+
+typedef struct unc_events unc_events;
+int unc_event_params_default(unc_event_params *p);
+/* model_table_path: 1024 x {mean, stdv} f32, template order (uncalled_b200/data/r94_5mer_template.f32 is the built-in
+ * r9.4 model).  The device is the one selected by unc_init.  UNC_E_NO_DEVICE without a CUDA device. */
+int unc_events_create(const char *model_table_path, const unc_event_params *prm, unc_events **out);
+void unc_events_free(unc_events *h);
+/* Synchronous.  samples_on_device: `samples` is a device pointer on the handle's device.  out[i]: read i's counts and
+ * normaliser; the events stay on the device until unc_events_fetch or the next run. */
+int unc_events_run(unc_events *h, const unc_read_desc *reads, uint32_t n_reads, const void *samples, int samples_on_device,
+                   unc_event_read *out);
+/* out: room for the sum of the last run's n_events; read i's events follow read i-1's. */
+int unc_events_fetch(unc_events *h, unc_event_full *out);
+/* The caller's event means: read i is means[off[i] .. off[i+1]).  Writes norm_mean, win_mean, win_stdv, win_mask of
+ * each mean at the mean's own index (entries off[0] .. off[n_reads] of each array; any may be NULL) and scale / shift
+ * per read (n_reads entries; may be NULL). */
+int unc_events_annotate(unc_events *h, uint32_t n_reads, const uint64_t *off, const float *means, float *norm_mean,
+                        float *win_mean, float *win_stdv, uint32_t *win_mask, float *scale, float *shift);
+/* out[i * 1024 + k] = Mapper::model.match_prob(means[i], k): the model as the mapper holds it (pmodel_r94_complement,
+ * src/mapper.cpp:57, built from the table as unc_index_load builds it), bit for bit what unc_match_probs returns for k. */
+int unc_match_probs_batch(unc_events *h, const float *means, uint64_t n, float *out);
+/* CUDA-event times of the last run in ms: H2D, detection, normaliser + profiler, D2H of the per-read results. */
+int unc_events_last_times(const unc_events *h, float ms[4]);
 
 /* ---- resource accounting (tests) -----------------------------------------------------------------------------
  * What the library holds at this moment: bytes of device memory, bytes of pinned host memory, and CUDA streams plus

@@ -9,3 +9,4 @@ from .mask import mask_external, mask_internal  # noqa: F401
 __version__ = "0.1.0"
 from .dtw import (DTW_EVENT_GLOB, DTW_EVENT_QSUB, DTW_EVENT_RSUB, DTW_RAW_GLOB, DTW_RAW_QSUB, DTW_RAW_RSUB,  # noqa: F401
                   DTWParams, DTWr94d, DTWr94p, DTWSubSeq, dtw_batch)
+from .signal import EventBatch, SignalProcessor, annotate, detect_events, match_probs, normalize  # noqa: F401

@@ -35,6 +35,14 @@ class Params(C.Structure):
                 ("bp_per_sec", C.c_float), ("sample_rate", C.c_float)]
 
 
+class EventParams(C.Structure):
+    """unc_event_params: EventDetector::Params and EventProfiler's win_len / win_stdv_min (reference
+    src/event_detector.cpp:17-26, src/event_profiler.cpp:3-9)."""
+    _fields_ = [("window_length1", C.c_uint32), ("window_length2", C.c_uint32), ("threshold1", C.c_float),
+                ("threshold2", C.c_float), ("peak_height", C.c_float), ("min_mean", C.c_float), ("max_mean", C.c_float),
+                ("win_len", C.c_uint32), ("win_stdv_min", C.c_float)]
+
+
 class ReadDesc(C.Structure):
     _fields_ = [("offset", C.c_uint64), ("n_samples", C.c_uint32), ("dtype", C.c_uint32),
                 ("cal_range", C.c_float), ("cal_offset", C.c_float), ("cal_digit", C.c_float)]
@@ -89,7 +97,9 @@ EXPORTS = ["unc_strerror", "unc_last_error", "unc_device_count", "unc_init", "un
            "unc_mask_external_last_times", "unc_index_build_device", "unc_index_build_device_last_times",
            "unc_index_build_device_last_active", "unc_dtw_aligner_create", "unc_dtw_aligner_free", "unc_dtw_aligner_contig",
            "unc_dtw_aligner_set_budget", "unc_dtw_align_batch", "unc_dtw_align_path", "unc_dtw_align_last_times",
-           "unc_debug_held", "unc_dtw_batch_banded", "unc_dtw_aligner_set_band"]
+           "unc_debug_held", "unc_dtw_batch_banded", "unc_dtw_aligner_set_band", "unc_event_params_default", "unc_events_create",
+           "unc_events_free", "unc_events_run", "unc_events_fetch", "unc_events_annotate", "unc_match_probs_batch",
+           "unc_events_last_times"]
 
 
 def build(force=False, verbose=False):
@@ -97,7 +107,7 @@ def build(force=False, verbose=False):
     src_dir = os.path.join(PKG_DIR, "csrc")
     srcs = [os.path.join(src_dir, f) for f in ("unc_abi.cu", "unc_index_build.cpp", "unc_fast5.cpp")]
     deps = srcs + [os.path.join(src_dir, f) for f in
-                   ("unc_device.cuh", "unc_k2v2.cuh", "unc_dtw.cuh", "unc_dtw_band.cuh", "unc_dtw_host.inl", "unc_dtw_align.cuh", "unc_dtw_align_host.inl", "unc_k1.cuh", "unc_stream.cuh", "unc_stream_host.inl", "unc_stream_logic.hpp", "unc_replay.cuh", "unc_replay_host.inl", "unc_ordered_logic.hpp", "unc_pdqsort.cuh", "unc_warp.cuh",
+                   ("unc_device.cuh", "unc_k2v2.cuh", "unc_dtw.cuh", "unc_dtw_band.cuh", "unc_dtw_host.inl", "unc_dtw_align.cuh", "unc_dtw_align_host.inl", "unc_k1.cuh", "unc_stream.cuh", "unc_stream_host.inl", "unc_stream_logic.hpp", "unc_replay.cuh", "unc_replay_host.inl", "unc_events.cuh", "unc_events_host.inl", "unc_ordered_logic.hpp", "unc_pdqsort.cuh", "unc_warp.cuh",
                     "unc_selfalign.cuh", "unc_selfalign_host.hpp", "unc_selfalign_host.inl",
                     "unc_mask.cuh", "unc_mask_host.hpp", "unc_mask_host.inl",
                     "unc_mask_ext.cuh", "unc_mask_ext_host.hpp", "unc_mask_ext_host.inl",
@@ -220,6 +230,15 @@ def lib():
     L.unc_dtw_align_path.argtypes = [vp, u32, vp, vp, vp]
     L.unc_dtw_align_last_times.argtypes = [vp, vp, C.POINTER(u64), C.POINTER(u64)]
     L.unc_debug_held.argtypes = [C.POINTER(u64), C.POINTER(u64), C.POINTER(u32)]
+    L.unc_event_params_default.argtypes = [C.POINTER(EventParams)]
+    L.unc_events_create.argtypes = [C.c_char_p, C.POINTER(EventParams), C.POINTER(vp)]
+    L.unc_events_free.argtypes = [vp]
+    L.unc_events_free.restype = None
+    L.unc_events_run.argtypes = [vp, vp, u32, vp, C.c_int, vp]
+    L.unc_events_fetch.argtypes = [vp, vp]
+    L.unc_events_annotate.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.unc_match_probs_batch.argtypes = [vp, vp, u64, vp]
+    L.unc_events_last_times.argtypes = [vp, C.POINTER(C.c_float)]
     _lib = L
     return L
 

@@ -8,7 +8,11 @@ import os
 import sys
 import time
 
+import numpy as np
+
 MAX_SLEEP = 0.01
+EVENTS_COLUMNS = ("read_id", "start", "length", "mean", "stdv", "norm_scale", "norm_shift", "norm_mean", "win_mean",
+                  "win_stdv", "win_mask")
 
 
 def get_parser(conf):
@@ -131,6 +135,22 @@ def get_parser(conf):
     p.add_argument("--band", type=int, default=0, help="Align within this many rows (k-mers) of the diagonal instead of "
                    "the whole matrix (0: the whole matrix, and reads over 50 000 kept means are skipped)")
     p.add_argument("-r", "--recursive", action="store_true", help="Recursively search 'fast5s' for fast5 files")
+    p.add_argument("--device", type=int, default=0, help="CUDA device")
+
+    p = sp.add_parser("events", help="Write every event of every read with the mapper's normalisation and stall mask "
+                      "(the reference's DEBUG_EVENTS columns) as one TSV on stdout", formatter_class=fmt,
+                      description="One row per event, reads in input order, columns: " + " ".join(EVENTS_COLUMNS) + ". "
+                      "Floats are printed with %%.9g so that they read back to the same float32 (the reference's "
+                      "debug file prints 6 significant digits).  win_mean and win_stdv are nan for the last events of "
+                      "a read, which never reach the middle of the profiler's window.  The whole signal is used.")
+    p.add_argument("fast5s", nargs="+", type=str, help="Reads. Can be a directory which will be searched for all files with "
+                   "the \".fast5\" extension, a text file containing one fast5 filename per line, or a fast5 file.")
+    p.add_argument("-r", "--recursive", action="store_true", help="Recursively search 'fast5s' for fast5 files")
+    p.add_argument("-l", "--read-list", type=str, default=None, help="Only write reads listed in this file")
+    p.add_argument("-n", "--max-reads", type=int, default=None, help="Maximum number of reads to write")
+    p.add_argument("--model", type=str, default=None, help="Pore model table (1024 x {mean, stdv} float32, template "
+                   "k-mer order); default: the built-in r9.4 model")
+    p.add_argument("--batch-reads", type=int, default=256, help="Reads per GPU batch")
     p.add_argument("--device", type=int, default=0, help="CUDA device")
 
     p = sp.add_parser("pafstats",help="Computes speed and accuracy of UNCALLED mappings.", formatter_class=fmt)
@@ -333,6 +353,90 @@ def dtw_cmd(args, out=None):
             out.flush()
 
 
+def events_cmd(args, out=None):
+    """`events`: every event of the selected reads (uncalled_b200.signal) as TSV on `out` (stdout).  The next batch is
+    decoded on a host thread while the GPU processes this one.  A bad argument or a missing file ends the command with
+    status 1 before the GPU is touched."""
+    from concurrent.futures import ThreadPoolExecutor
+    from .fast5 import Fast5File
+    from .signal import SignalProcessor
+    out = out or sys.stdout
+    if args.max_reads is not None and args.max_reads < 0:
+        sys.stderr.write("Error: --max-reads must not be negative\n")
+        sys.exit(1)
+    if args.batch_reads < 1:
+        sys.stderr.write("Error: --batch-reads must be at least 1\n")
+        sys.exit(1)
+    if args.device < 0:
+        sys.stderr.write("Error: --device must not be negative\n")
+        sys.exit(1)
+    if args.model is not None:
+        assert_exists(args.model)
+        if os.path.getsize(args.model) != 1024 * 2 * 4:
+            sys.stderr.write("Error: '%s' is not a pore model table of 1024 (mean, stdv) float32 pairs\n" % args.model)
+            sys.exit(1)
+    ids = None
+    if args.read_list:
+        assert_exists(args.read_list)
+        ids = set(l.strip() for l in open(args.read_list) if l.strip())
+    files = [f for f in load_fast5s(args.fast5s, args.recursive) if f is not None]
+    cap = args.max_reads or 0
+
+    def batches():
+        """the selected reads, whole signals, in file order, batch_reads at a time"""
+        batch, n = [], 0
+        for path in files:
+            with Fast5File(path) as f:
+                for i in range(f.n_reads):
+                    if cap and n >= cap:
+                        break
+                    if ids is not None and f.info(i).read_id not in ids:
+                        continue
+                    batch.append(f.load(i, 1)[0])
+                    n += 1
+                    if len(batch) >= args.batch_reads:
+                        yield batch
+                        batch = []
+            if cap and n >= cap:
+                break
+        if batch:
+            yield batch
+
+    out.write("\t".join(EVENTS_COLUMNS) + "\n")
+    proc = None
+    with ThreadPoolExecutor(max_workers=1) as ex:
+        it = batches()
+        fut = ex.submit(next, it, None)
+        while True:
+            batch = fut.result()
+            if batch is None:
+                break
+            fut = ex.submit(next, it, None)
+            if proc is None:
+                proc = SignalProcessor(model_path=args.model, device=args.device)
+            res = proc.run([r.signal for r in batch], [r.calibration for r in batch])
+            out.write(format_events([r.read_id for r in batch], res))
+            out.flush()
+
+
+def _g9(a):
+    """%.9g of every value of a float32 array (reads back to the same float32), as a list of strings"""
+    return ["%.9g" % x for x in np.asarray(a, np.float64).tolist()]
+
+
+def format_events(read_ids, res):
+    """TSV rows of an EventBatch (EVENTS_COLUMNS without the header), formatted column by column"""
+    ev = res.events
+    if ev is None or len(ev) == 0:
+        return ""
+    n = res.reads["n_events"].astype(np.int64)
+    per_read = lambda v: np.repeat(np.asarray(v, dtype=object), n).tolist()   # noqa: E731
+    cols = [per_read(list(read_ids)), ev["start"].astype(str).tolist(), _g9(ev["length"]), _g9(ev["mean"]),
+            _g9(ev["stdv"]), per_read(_g9(res.reads["norm_scale"])), per_read(_g9(res.reads["norm_shift"])),
+            _g9(ev["norm_mean"]), _g9(ev["win_mean"]), _g9(ev["win_stdv"]), ev["win_mask"].astype(str).tolist()]
+    return "".join("\t".join(row) + "\n" for row in zip(*cols))
+
+
 def load_conf(argv):
     """uncalled/args.py:288-302: every parsed option whose name is a Conf attribute is set on the Conf."""
     from .api import Conf
@@ -373,6 +477,8 @@ def main(argv=None):
         sys.stdout.write("Masked %d basepairs\n" % masked)
     elif args.subcmd == "dtw":
         dtw_cmd(args)
+    elif args.subcmd == "events":
+        events_cmd(args)
     elif args.subcmd == "pafstats":
         from . import pafstats
         pafstats.run(args.infile, args.ref_paf, args.max_reads)

@@ -415,6 +415,108 @@ struct ClientSim {
     explicit ClientSim(Conf &) { throw std::runtime_error("ClientSim (`uncalled sim`) is outside the scope of this module"); }
 };
 
+// ------------------------------------------------------------------ signal front end (reference src/pybinder.cpp:44-56)
+// Event, EventDetector, EventProfiler and PoreModel with the reference's names, computed by the `events` kernels
+// (unc_events_*).  Only whole-signal / whole-read methods are offered: the per-sample and streaming ones (add_sample,
+// add_event, Normalizer push / pop) would cost one GPU launch per sample or event and are deliberately left out.
+struct Event { float mean = 0, stdv = 0; u32 start = 0, length = 0; };   // src/event_detector.hpp:19-24
+
+static unc_events *events_create(const unc_event_params &p) {
+    unc_events *h = nullptr;
+    check(unc_events_create(Engine::default_model_table().c_str(), &p, &h), "unc_events_create");
+    return h;
+}
+
+// EventDetector (src/event_detector.cpp:17-153): get_events / get_means over a whole signal, mean_event_len of the last
+class EventDetector {
+    unc_event_params prm_;
+    unc_events *h_ = nullptr;
+    float mel_ = NAN;
+    std::vector<unc_event_full> run(const std::vector<float> &raw) {
+        if (!h_) h_ = events_create(prm_);
+        unc_read_desc d = {0, (u32) raw.size(), UNC_DTYPE_F32, 1.0f, 0.0f, 1.0f};
+        unc_event_read r;
+        std::vector<float> buf(raw.empty() ? 1 : raw.size());
+        std::copy(raw.begin(), raw.end(), buf.begin());
+        check(unc_events_run(h_, &d, 1, buf.data(), 0, &r), "unc_events_run");
+        std::vector<unc_event_full> ev(r.n_events);
+        if (r.n_events) check(unc_events_fetch(h_, ev.data()), "unc_events_fetch");
+        mel_ = r.mean_event_len;
+        return ev;
+    }
+  public:
+    EventDetector() { unc_event_params_default(&prm_); }
+    explicit EventDetector(const unc_event_params &p) : prm_(p) {
+        if (p.window_length1 != 3 || p.window_length2 != 6) throw std::invalid_argument("window lengths are fixed at 3 and 6");
+    }
+    ~EventDetector() { if (h_) unc_events_free(h_); }
+    EventDetector(const EventDetector &) = delete;
+    std::vector<Event> get_events(const std::vector<float> &raw) {
+        std::vector<Event> out;
+        for (const unc_event_full &e : run(raw)) out.push_back(Event{e.mean, e.stdv, e.start, (u32) e.length});
+        return out;
+    }
+    std::vector<float> get_means(const std::vector<float> &raw) {
+        std::vector<float> out;
+        for (const unc_event_full &e : run(raw)) out.push_back(e.mean);
+        return out;
+    }
+    float mean_event_len() const { return mel_; }
+};
+
+// EventProfiler (src/event_profiler.hpp:14-151, defaults src/event_profiler.cpp:3-9): get_full_mask over given events
+class EventProfiler {
+    unc_events *h_ = nullptr;
+  public:
+    EventProfiler() = default;
+    ~EventProfiler() { if (h_) unc_events_free(h_); }
+    EventProfiler(const EventProfiler &) = delete;
+    std::vector<bool> get_full_mask(const std::vector<Event> &events) {
+        if (!h_) { unc_event_params p; unc_event_params_default(&p); h_ = events_create(p); }
+        std::vector<float> means(events.size() + 1);
+        for (size_t i = 0; i < events.size(); i++) means[i] = events[i].mean;
+        const uint64_t off[2] = {0, events.size()};
+        std::vector<uint32_t> mask(events.size() + 1);
+        check(unc_events_annotate(h_, 1, off, means.data(), nullptr, nullptr, nullptr, mask.data(), nullptr, nullptr),
+              "unc_events_annotate");
+        return std::vector<bool>(mask.begin(), mask.begin() + events.size());
+    }
+};
+
+// PoreModel (src/pore_model.hpp:163-165): match_prob of the r9.4 model in template or complement k-mer order (the
+// mapper holds the complement one, src/mapper.cpp:57)
+class PoreModel {
+    bool complement_;
+    unc_events *h_ = nullptr;
+  public:
+    explicit PoreModel(bool complement) : complement_(complement) {}
+    ~PoreModel() { if (h_) unc_events_free(h_); }
+    PoreModel(const PoreModel &o) : complement_(o.complement_) {}
+    py::array_t<float> match_probs(py::array_t<float, py::array::c_style | py::array::forcecast> means) {
+        if (!h_) { unc_event_params p; unc_event_params_default(&p); h_ = events_create(p); }
+        const uint64_t n = (uint64_t) means.size();
+        py::array_t<float> dev({(py::ssize_t) n, (py::ssize_t) 1024});
+        if (n) check(unc_match_probs_batch(h_, means.data(), n, dev.mutable_data()), "unc_match_probs_batch");
+        if (complement_) return dev;
+        // the device table is in complement order: template k-mer k sits at k ^ 0x3FF (src/bp.hpp:77-80)
+        py::array_t<float> out({(py::ssize_t) n, (py::ssize_t) 1024});
+        for (uint64_t i = 0; i < n; i++)
+            for (u32 k = 0; k < 1024; k++) out.mutable_data()[i * 1024 + k] = dev.data()[i * 1024 + (k ^ 0x3FFu)];
+        return out;
+    }
+    float match_prob(float samp, u16 kmer) {
+        if (kmer >= 1024) throw std::invalid_argument("k-mer out of range");
+        py::array_t<float> m(1);
+        m.mutable_data()[0] = samp;
+        return match_probs(m).data()[kmer];
+    }
+};
+
+static u32 fixed_window(u32 v, u32 want) {
+    if (v != want) throw std::invalid_argument("the event window lengths are fixed at 3 and 6 on the device");
+    return v;
+}
+
 #define PRP(N, DOC) conf.def_readwrite(#N, &Conf::N, DOC)
 
 PYBIND11_MODULE(_uncalled, m) {
@@ -517,4 +619,34 @@ PYBIND11_MODULE(_uncalled, m) {
     m.attr("DTW_EVENT_RSUB") = py::cast(DTW_EVENT_RSUB);
     m.attr("DTW_RAW_QSUB") = py::cast(DTW_EVENT_QSUB);        // as bound by the reference (src/pybinder.cpp:90-91): the EVENT presets
     m.attr("DTW_RAW_RSUB") = py::cast(DTW_EVENT_RSUB);
+    py::class_<Event>(m, "Event")
+        .def(py::init<>())
+        .def_readwrite("mean", &Event::mean).def_readwrite("stdv", &Event::stdv)
+        .def_readwrite("start", &Event::start).def_readwrite("length", &Event::length);
+    py::class_<EventDetector> evd(m, "EventDetector", "EventDetector on the GPU: get_events / get_means over whole signals. "
+                                  "add_sample is not offered (one GPU launch per sample).");
+    py::class_<unc_event_params>(evd, "Params")
+        .def(py::init([]() { unc_event_params p; unc_event_params_default(&p); return p; }))
+        .def_property("window_length1", [](const unc_event_params &p) { return p.window_length1; },
+                      [](unc_event_params &p, u32 v) { p.window_length1 = fixed_window(v, 3); })
+        .def_property("window_length2", [](const unc_event_params &p) { return p.window_length2; },
+                      [](unc_event_params &p, u32 v) { p.window_length2 = fixed_window(v, 6); })
+        .def_readwrite("threshold1", &unc_event_params::threshold1).def_readwrite("threshold2", &unc_event_params::threshold2)
+        .def_readwrite("peak_height", &unc_event_params::peak_height).def_readwrite("min_mean", &unc_event_params::min_mean)
+        .def_readwrite("max_mean", &unc_event_params::max_mean);
+    evd.def(py::init<>()).def(py::init<const unc_event_params &>())
+        .def("get_events", &EventDetector::get_events)
+        .def("get_means", &EventDetector::get_means)
+        .def("mean_event_len", &EventDetector::mean_event_len);
+    py::class_<EventProfiler>(m, "EventProfiler", "EventProfiler on the GPU: get_full_mask over a read's events. "
+                              "add_event / anno_event are not offered (one GPU launch per event).")
+        .def(py::init<>())
+        .def("get_full_mask", &EventProfiler::get_full_mask);
+    py::class_<PoreModel>(m, "PoreModel", "The r9.4 pore model on the GPU: match_prob of one mean, or of an array of "
+                          "means against all 1024 k-mers")
+        .def(py::init<bool>(), py::arg("complement") = true)
+        .def("match_prob", &PoreModel::match_prob)
+        .def("match_prob", &PoreModel::match_probs);
+    m.attr("pmodel_r94_template") = py::cast(PoreModel(false));
+    m.attr("pmodel_r94_complement") = py::cast(PoreModel(true));
 }

@@ -963,3 +963,4 @@ int unc_debug_held(uint64_t *device_bytes, uint64_t *pinned_bytes, uint32_t *han
 #include "unc_mask_host.inl"
 #include "unc_mask_ext_host.inl"
 #include "unc_fmb_host.inl"
+#include "unc_events_host.inl"

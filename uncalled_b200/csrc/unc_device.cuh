@@ -381,9 +381,14 @@ UNC_DEV void unc_evdt_reset(DevEvdt &e) {
     e.ld = e.sd;
 }
 
+struct DevEvdtFull { float mean, stdv; u32 start, length; };   // Event (reference src/event_detector.hpp:19-24)
+
 // reference src/event_detector.cpp:83-112 (add_sample) + :296-319 (create_event).
 // Returns true and sets *mean when a valid event (min_mean <= mean <= max_mean) is emitted.
-UNC_DEV bool unc_evdt_add(DevEvdt &e, const DevParams &p, float s, float *mean_out) {
+// FULL (the `events` kernels, unc_events.cuh) also fills *full with the whole Event of every emitted event; the
+// mapper's instantiation (FULL = false) computes only the mean.
+template <bool FULL = false>
+UNC_DEV bool unc_evdt_add(DevEvdt &e, const DevParams &p, float s, float *mean_out, DevEvdtFull *full = nullptr) {
     u32 t_mod = e.t % 13u;
     u32 prev = t_mod > 0 ? t_mod - 1 : 12u;
     float ss = f_mul(s, s);
@@ -400,6 +405,16 @@ UNC_DEV bool unc_evdt_add(DevEvdt &e, const DevParams &p, float s, float *mean_o
     u32 eb = evt_en % 13u;
     u32 length = (u32) (float) (evt_en - e.evt_st);
     float mean = (float) d_div(d_sub(e.sum[eb], e.evt_st_sum), (double) length);
+    if (FULL) {
+        // deltasqr: the double difference rounded to float; var: float arithmetic (length u32 -> float); then
+        // calibrate(), which is (v + 0) * 1 for the detector's default calibration: the samples arrive calibrated
+        const float deltasqr = (float) d_sub(e.sumsq[eb], e.evt_st_sumsq);
+        const float var = f_sub(f_div(deltasqr, (float) length), f_mul(mean, mean));
+        full->stdv = f_mul(f_add(f_sqrt(fmaxf(var, 0.0f)), 0.0f), 1.0f);
+        full->mean = f_mul(f_add(mean, 0.0f), 1.0f);
+        full->start = e.evt_st;
+        full->length = length;
+    }
     e.evt_st = evt_en;
     e.evt_st_sum = e.sum[eb];
     e.evt_st_sumsq = e.sumsq[eb];

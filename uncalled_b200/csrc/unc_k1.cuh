@@ -199,7 +199,10 @@ UNC_DEV bool k1_exact_ok(float tot, u32 mn, i32 emin_floor) {
 // the class window holds D3[m-6], D3[m-3], D3[m]; the step adds D3[m+3] and shifts.  Window sums
 // (reference src/event_detector.cpp:195-205, differences of the double prefix sums -- exact here):
 //   w=3: left D3[m-3], right D3[m];   w=6: left D3[m-6]+D3[m-3], right D3[m]+D3[m+3].
-UNC_DEV void k1_tpass(K1WarpSmem *sm, const K1Read &R, const K1Tile &T, i32 a, int lane, double *chunk_sum, K1Exact &X) {
+// FULL (the `events` kernels): *chunk_sq also receives the sum of the chunk's float squares.
+template <bool FULL = false>
+UNC_DEV void k1_tpass(K1WarpSmem *sm, const K1Read &R, const K1Tile &T, i32 a, int lane, double *chunk_sum, K1Exact &X,
+                      double *chunk_sq = nullptr) {
     double D[3][3], E[3][3];
     double p2, p1, r2, r1;
     {
@@ -219,7 +222,7 @@ UNC_DEV void k1_tpass(K1WarpSmem *sm, const K1Read &R, const K1Tile &T, i32 a, i
         }
         p2 = xd[9]; p1 = xd[10]; r2 = qd[9]; r1 = qd[10];
     }
-    double acc = 0.0;
+    double acc = 0.0, acc2 = 0.0;
     float *row1 = sm->t1 + (u32) lane * K1_TS, *row2 = sm->t2 + (u32) lane * K1_TS;
 #pragma unroll 1
     for (u32 i0 = 0; i0 < K1_CH; i0 += 3) {
@@ -237,6 +240,7 @@ UNC_DEV void k1_tpass(K1WarpSmem *sm, const K1Read &R, const K1Tile &T, i32 a, i
             float v1 = k1_tstat<3>(D[c][1], E[c][1], D[c][2], E[c][2]);
             float v2 = k1_tstat<6>(d_add(D[c][0], D[c][1]), d_add(E[c][0], E[c][1]), d_add(D[c][2], dn), d_add(E[c][2], en));
             if (c == 0) acc = d_add(acc, D[c][2]);           // samples m, m+1, m+2
+            if (FULL && c == 0) acc2 = d_add(acc2, E[c][2]);
             D[c][0] = D[c][1]; D[c][1] = D[c][2]; D[c][2] = dn;
             E[c][0] = E[c][1]; E[c][1] = E[c][2]; E[c][2] = en;
             row1[i0 + c] = v1;
@@ -244,6 +248,7 @@ UNC_DEV void k1_tpass(K1WarpSmem *sm, const K1Read &R, const K1Tile &T, i32 a, i
         }
     }
     *chunk_sum = acc;
+    if (FULL) *chunk_sq = acc2;
 }
 
 // t-statistics of the first positions, where the reference's ring indices wrap (u32 buf_mid - w
@@ -289,8 +294,23 @@ struct K1Carry {                   // warp-uniform state carried across the tile
     K1Exact X;
 };
 
+// Where the FULL variant (the `events` kernels, unc_events.cuh) writes read r's events: slots row[r] .. of each array.
+// The prefix sums of the float squares at the fired peaks go to a list of its own, `sql` (K1_CH entries of 2 words per
+// lane), next to the prefix sums of the samples in the lane's T rows.
+struct K1FullOut {
+    const u64 *row;
+    u32 *start;
+    float *length, *mean, *stdv;
+};
+#define K1_SQL_WORDS (32u * 2u * K1_CH)   /* words of `sql` per warp */
+
 // One read by one warp.  Returns false when the read must be redone by the serial routine.
-UNC_DEV bool k1_warp_read(const DevBatch &B, const DevParams &p, u32 r, K1WarpSmem *sm, u32 *bar_phase) {
+// FULL: every event (start, length, mean, stdv: reference src/event_detector.cpp:296-319) goes to *fo instead of the
+// mean to B.events.  The sums of squares are exact under the same condition as the sums (k1_exact_ok checks both), so
+// the same flag sends a read to the serial routine.
+template <bool FULL = false>
+UNC_DEV bool k1_warp_read(const DevBatch &B, const DevParams &p, u32 r, K1WarpSmem *sm, u32 *bar_phase,
+                          const K1FullOut *fo = nullptr, u32 *sql = nullptr) {
     u32 *stats = B.k1_stats;
     const int lane = w_lane();
     const DevReadDesc rd = B.reads[r];
@@ -314,6 +334,7 @@ UNC_DEV bool k1_warp_read(const DevBatch &B, const DevParams &p, u32 r, K1WarpSm
     C.fsm.l_masked = 0; C.fsm.l_pos = -1; C.fsm.l_val = 0.0f; C.fsm.l_valid = 0;
     C.base = 0.0; C.evt_st = 0; C.evt_st_sum = 0.0; C.ne = 0; C.total_events = 0; C.len_total = 0;
     C.X.sum = 0.0f; C.X.sum2 = 0.0f; C.X.mn = 0xFFFFFFFFu; C.X.mn2 = 0xFFFFFFFFu;
+    double base2 = 0.0, evt_st_sq = 0.0;                           // FULL: the same two carries for the squares
     bool ok = R.n < (1u << 24);
     const u32 n_tiles = ok ? (R.n_pos + K1_TILE - 1u) / K1_TILE : 0u;
 
@@ -345,8 +366,8 @@ UNC_DEV bool k1_warp_read(const DevBatch &B, const DevParams &p, u32 r, K1WarpSm
         // ---- T pass
         const i32 a = (i32) (lo + (u32) lane * K1_CH);
         const u32 steps = (u32) a >= R.n_pos ? 0u : (R.n_pos - (u32) a < K1_CH ? R.n_pos - (u32) a : K1_CH);
-        double csum = 0.0;
-        if (steps) k1_tpass(sm, R, T, a, lane, &csum, C.X);
+        double csum = 0.0, csq = 0.0;
+        if (steps) k1_tpass<FULL>(sm, R, T, a, lane, &csum, C.X, &csq);
         w_sync();
         if (t == 0 && lane == 0) k1_fix_head(sm, R, T);
         w_sync();
@@ -358,6 +379,16 @@ UNC_DEV bool k1_warp_read(const DevBatch &B, const DevParams &p, u32 r, K1WarpSm
         }
         const double lane_base = d_add(C.base, d_sub(incl, csum));
         const double tile_sum = u2d(w_shfl64(d2u(incl), 31));
+        double lane_base2 = 0.0, tile_sum2 = 0.0;
+        if (FULL) {
+            double incl2 = csq;
+            for (int d = 1; d < 32; d <<= 1) {
+                double y = u2d(w_shfl_up64(d2u(incl2), d));
+                if (lane >= d) incl2 = d_add(incl2, y);
+            }
+            lane_base2 = d_add(base2, d_sub(incl2, csq));
+            tile_sum2 = u2d(w_shfl64(d2u(incl2), 31));
+        }
 
         // ---- speculative FSM
         K1Fsm sigma, phi;
@@ -391,15 +422,30 @@ UNC_DEV bool k1_warp_read(const DevBatch &B, const DevParams &p, u32 r, K1WarpSm
             double q0 = lane_base, q1 = lane_base, q2 = lane_base;
             if (a >= 1) { q1 = d_sub(q0, (double) k1_sample(sm, R, T, a - 1)); q2 = q1; }
             if (a >= 2) q2 = d_sub(q1, (double) k1_sample(sm, R, T, a - 2));
+            double g0 = lane_base2, g1 = lane_base2, g2 = lane_base2;      // FULL: the same for the squares
+            if (FULL) {
+                if (a >= 1) { float x = k1_sample(sm, R, T, a - 1); g1 = d_sub(g0, (double) f_mul(x, x)); g2 = g1; }
+                if (a >= 2) { float x = k1_sample(sm, R, T, a - 2); g2 = d_sub(g1, (double) f_mul(x, x)); }
+            }
             for (u32 i = 0; i < steps; i++) {
                 if ((fires >> i) & 1ull) {                   // the event ends at buf_mid - w1 + 1 = m - 2 (:105)
                     u64 bits = d2u(q2);
                     u32 *e = k1_list(sm, lane, cnt);
                     e[0] = (u32) bits; e[1] = (u32) (bits >> 32);
+                    if (FULL) {
+                        u64 b2 = d2u(g2);
+                        u32 *f = sql + (u32) lane * (2u * K1_CH) + 2u * cnt;
+                        f[0] = (u32) b2; f[1] = (u32) (b2 >> 32);
+                    }
                     cnt++;
                 }
                 q2 = q1; q1 = q0;
                 q0 = d_add(q0, (double) k1_sample(sm, R, T, a + (i32) i));
+                if (FULL) {
+                    float x = k1_sample(sm, R, T, a + (i32) i);
+                    g2 = g1; g1 = g0;
+                    g0 = d_add(g0, (double) f_mul(x, x));
+                }
             }
         }
         w_sync();
@@ -407,20 +453,26 @@ UNC_DEV bool k1_warp_read(const DevBatch &B, const DevParams &p, u32 r, K1WarpSm
 
         // ---- events: each fired peak closes the event opened by the previous one (create_event :296-319)
         // previous fire before this lane's first: nearest earlier lane with a fire, else the carry
-        u32 lp = 0; u64 ls = 0;
+        u32 lp = 0; u64 ls = 0, ls2 = 0;
         if (cnt) {
             lp = (u32) a + (u32) (63 - d_clzll(fires)) - 2u;
             const u32 *e = k1_list(sm, lane, cnt - 1);
             ls = (u64) e[1] << 32 | e[0];
+            if (FULL) { const u32 *f = sql + (u32) lane * (2u * K1_CH) + 2u * (cnt - 1); ls2 = (u64) f[1] << 32 | f[0]; }
         }
         u32 has = cnt ? 1u : 0u;
         for (int d = 1; d < 32; d <<= 1) {                   // inclusive "last fire so far" scan
             u32 oh = w_shfl_up(has, d), op = w_shfl_up(lp, d); u64 os = w_shfl_up64(ls, d);
-            if (lane >= d && !has && oh) { has = 1u; lp = op; ls = os; }
+            u64 os2 = FULL ? w_shfl_up64(ls2, d) : 0ull;
+            if (lane >= d && !has && oh) { has = 1u; lp = op; ls = os; if (FULL) ls2 = os2; }
         }
         u32 ph = w_shfl_up(has, 1), pp = w_shfl_up(lp, 1); u64 ps = w_shfl_up64(ls, 1);
         u32 st_pos = (lane > 0 && ph) ? pp : C.evt_st;
         double st_sum = (lane > 0 && ph) ? u2d(ps) : C.evt_st_sum;
+        double st_sq = 0.0;
+        if (FULL) { u64 ps2 = w_shfl_up64(ls2, 1); st_sq = (lane > 0 && ph) ? u2d(ps2) : evt_st_sq; }
+        const u32 st_pos0 = st_pos;
+        const double st_sum0 = st_sum;
         const u32 maxcnt = w_max(cnt);
         u32 nvalid = 0, len_acc = 0;
         u64 fl = fires;
@@ -433,17 +485,49 @@ UNC_DEV bool k1_warp_read(const DevBatch &B, const DevParams &p, u32 r, K1WarpSm
                 u32 length = en - st_pos;
                 float mean = (float) d_div(d_sub(en_sum, st_sum), (double) length);
                 len_acc += length;
-                if (mean >= p.min_mean && mean <= p.max_mean) { k1_list(sm, lane, nvalid)[0] = f2u(mean); nvalid++; }
+                if (mean >= p.min_mean && mean <= p.max_mean) { if (!FULL) k1_list(sm, lane, nvalid)[0] = f2u(mean); nvalid++; }
                 st_pos = en; st_sum = en_sum;
             }
         }
         u32 tot_valid, off = w_exscan(nvalid, &tot_valid);
-        for (u32 i = 0; i < nvalid; i++) ev[C.ne + off + i] = u2f(k1_list(sm, lane, i)[0]);
+        if (!FULL) {
+            for (u32 i = 0; i < nvalid; i++) ev[C.ne + off + i] = u2f(k1_list(sm, lane, i)[0]);
+        } else {                                             // the lane's events again, now that their slots are known
+            u32 sp = st_pos0, k = C.ne + off;
+            double ss = st_sum0, sq = st_sq;
+            const u64 o = fo->row[r];
+            u64 f2 = fires;
+            for (u32 i = 0; i < cnt; i++) {
+                u32 bit = (u32) d_ctzll(f2); f2 &= f2 - 1;
+                u32 en = (u32) a + bit - 2u;
+                const u32 *e = k1_list(sm, lane, i);
+                const u32 *f = sql + (u32) lane * (2u * K1_CH) + 2u * i;
+                double en_sum = u2d((u64) e[1] << 32 | e[0]), en_sq = u2d((u64) f[1] << 32 | f[0]);
+                u32 length = en - sp;
+                float mean = (float) d_div(d_sub(en_sum, ss), (double) length);
+                if (mean >= p.min_mean && mean <= p.max_mean) {
+                    // create_event (:307-313): deltasqr rounded to float, var in float, calibrate() = (v + 0) * 1
+                    const float deltasqr = (float) d_sub(en_sq, sq);
+                    const float var = f_sub(f_div(deltasqr, (float) length), f_mul(mean, mean));
+                    fo->start[o + k] = sp;
+                    fo->length[o + k] = (float) length;
+                    fo->mean[o + k] = f_mul(f_add(mean, 0.0f), 1.0f);
+                    fo->stdv[o + k] = f_mul(f_add(f_sqrt(fmaxf(var, 0.0f)), 0.0f), 1.0f);
+                    k++;
+                }
+                sp = en; ss = en_sum; sq = en_sq;
+            }
+        }
         u32 tot_cnt, dummy = w_exscan(cnt, &tot_cnt); (void) dummy;
         u32 tot_len; dummy = w_exscan(len_acc, &tot_len);
         // carry
         u32 fh = w_shfl(has, 31), fp = w_shfl(lp, 31); u64 fs = w_shfl64(ls, 31);
         if (fh) { C.evt_st = fp; C.evt_st_sum = u2d(fs); }
+        if (FULL) {
+            u64 fs2 = w_shfl64(ls2, 31);
+            if (fh) evt_st_sq = u2d(fs2);
+            base2 = d_add(base2, tile_sum2);
+        }
         C.ne += tot_valid; C.total_events += tot_cnt; C.len_total += tot_len;
         C.base = d_add(C.base, tile_sum);
         w_sync();
@@ -496,8 +580,10 @@ UNC_DEV void unc_k1_norm_read(const DevBatch &B, const DevParams &p, u32 r) {
     B.shift[r] = shift;
 }
 
-// Warp body of the k1_events kernel: reads are pulled from an atomic queue.
-UNC_DEV void unc_k1_warp_main(const DevBatch &B, const DevParams &p, K1WarpSmem *sm) {
+// Warp body of the k1_events kernel (and, FULL, of k_events_warp): reads are pulled from an atomic queue.
+template <bool FULL = false>
+UNC_DEV void unc_k1_warp_main(const DevBatch &B, const DevParams &p, K1WarpSmem *sm, const K1FullOut *fo = nullptr,
+                              u32 *sql = nullptr) {
     const int lane = w_lane();
     if (lane == 0) t_bar_init(&sm->bar);
     w_sync();
@@ -507,6 +593,6 @@ UNC_DEV void unc_k1_warp_main(const DevBatch &B, const DevParams &p, K1WarpSmem 
         if (lane == 0) r = d_atomic_add(B.k1_queue, 1u);
         r = w_shfl(r, 0);
         if (r >= B.n_reads) break;
-        k1_warp_read(B, p, r, sm, &phase);
+        k1_warp_read<FULL>(B, p, r, sm, &phase, fo, sql);
     }
 }
