@@ -1,6 +1,7 @@
-"""Checkers of the banded DTW sweep (uncalled_b200/csrc/unc_dtw_band.cuh): the C restatement
-(oracle/unc_oracle_dtw_band.c orc_dtw_banded), the kernel source under the warp emulator (tests/emul/emul_dtw_band.cpp)
-and seeded problems that exercise the band's edges."""
+"""Checkers of the DTW sweeps (uncalled_b200/csrc/unc_dtw_band.cuh, unc_dtw.cuh): the C restatement of the band
+(oracle/unc_oracle_dtw_band.c orc_dtw_banded), the kernel sources under the warp emulator on the workspace plan of
+unc_dtw_plan.hpp (tests/emul/emul_dtw_band.cpp), an independent restatement of that plan's byte count, and seeded problems
+that exercise the band's edges."""
 import ctypes as C
 import os
 import subprocess
@@ -80,21 +81,26 @@ def emu():
         src = os.path.join(EMUL_DIR, "emul_dtw_band.cpp")
         out = os.path.join(EMUL_DIR, "libunc_emul_dtw_band.so")
         deps = [src, os.path.join(EMUL_DIR, "warp_emul.hpp")] + [os.path.join(CSRC, f) for f in (
-            "unc_dtw_band.cuh", "unc_dtw.cuh", "unc_device.cuh", "unc_warp.cuh")]
+            "unc_dtw_plan.hpp", "unc_dtw_band.cuh", "unc_dtw.cuh", "unc_device.cuh", "unc_warp.cuh")]
         if not (os.path.exists(out) and all(os.path.getmtime(out) >= os.path.getmtime(x) for x in deps)):
             subprocess.run(["g++", "-O2", "-g", "-std=c++17", "-ffp-contract=off", "-DUNC_EMUL", "-DK2_MAXSEG=16u", "-fPIC",
                             "-shared", "-I" + EMUL_DIR, "-I" + CSRC, "-o", out, src], check=True, capture_output=True)
         L = C.CDLL(out)
-        L.emu_dtw_sweep.argtypes = [vp, C.c_int, C.c_float, C.c_float, C.c_float, C.c_uint32, C.c_uint32] + [vp] * 9 + \
+        L.emu_dtw_sweep.argtypes = [vp, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_uint32, C.c_uint32] + [vp] * 9 + \
             [C.POINTER(C.c_uint64), C.c_int]
         L.emu_dtw_band_cells.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32]
         L.emu_dtw_band_cells.restype = C.c_uint64
+        L.emu_dtw_plan_bytes.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32]
+        L.emu_dtw_plan_bytes.restype = C.c_uint64
+        L.emu_dtw_pack.argtypes = [C.c_uint32, C.c_uint32, vp, vp, C.c_uint64, vp]
+        L.emu_dtw_pack.restype = C.c_uint32
         _emu = L
     return _emu
 
 
-def emulated(problems, band, cost_kind=0, w=(1.0, 1.0, 1.0), n_threads=64, want_bc=False):
-    """the kernel source under the emulator (band 0: k_dtw's full sweep): [(path, score, breadcrumbs or None)]"""
+def emulated(problems, band, cost_kind=0, w=(1.0, 1.0, 1.0), n_threads=64, want_bc=False, subseq=0):
+    """the kernel source under the emulator (band 0: k_dtw's full sweep, with subseq 0 NONE, 1 ROW or 2 COL):
+    [(path, score, breadcrumbs or None)]"""
     L = emu()
     n = len(problems)
     moff = np.zeros(n + 1, np.uint64)
@@ -111,7 +117,7 @@ def emulated(problems, band, cost_kind=0, w=(1.0, 1.0, 1.0), n_threads=64, want_
     sizes = [int(L.emu_dtw_band_cells(len(k), len(m), band)) if band else len(k) * len(m) for m, k in problems]
     bc = np.zeros(max(sum(sizes), 1), np.uint8) if want_bc else None
     nbc = C.c_uint64()
-    rc = L.emu_dtw_sweep(TAB.ctypes.data, cost_kind, w[0], w[1], w[2], band, n, am.ctypes.data, moff.ctypes.data, ak.ctypes.data,
+    rc = L.emu_dtw_sweep(TAB.ctypes.data, cost_kind, subseq, w[0], w[1], w[2], band, n, am.ctypes.data, moff.ctypes.data, ak.ctypes.data,
                          koff.ctypes.data, path.ctypes.data, poff.ctypes.data, plen.ctypes.data, score.ctypes.data,
                          None if bc is None else bc.ctypes.data, C.byref(nbc), n_threads)
     assert rc == 0
@@ -122,6 +128,50 @@ def emulated(problems, band, cost_kind=0, w=(1.0, 1.0, 1.0), n_threads=64, want_
         bo += sizes[i]
         out.append((path[int(poff[i]):int(poff[i]) + int(plen[i])].copy(), float(score[i]), b))
     return out
+
+
+SKIP = 0xFFFFFFFF
+
+
+def sweep_bytes(shapes, W):
+    """the span aligner's sweep workspace for problems [(R, C)] at half-width W (0: the full sweep), restated from the
+    kernels' needs: problem records (56 bytes), breadcrumbs (R x C, or the in-band cells), hrow / vcol / corners
+    (C + R + 3 ceil(R / 8) + 8 floats), the last column and row (R + C floats) or the column offsets (C + 1 u64), path room
+    (R + C pairs of u64), path lengths, scores, queue; each region 256-byte aligned"""
+    a = lambda x: (x + 255) // 256 * 256
+    n = len(shapes)
+    bc = diag = edge = path = 0
+    for R, C_ in shapes:
+        if W:
+            lo, hi = band_rows(R, C_, W)
+            bc += int((hi - lo + 1).sum())
+            edge += 8 * (C_ + 1)
+        else:
+            bc += R * C_
+            edge += 4 * (R + C_)
+        diag += 4 * (C_ + R + 3 * ((R + 7) // 8) + 8)
+        path += 16 * (R + C_)
+    return a(56 * n) + a(bc) + a(diag) + a(edge) + a(path) + a(8 * n) + a(4 * n) + a(4)
+
+
+def pack(shapes, W, budget):
+    """the span aligner's launches (dtw_pack) under the emulator: (launch of each problem or SKIP, number of launches)"""
+    rows = np.array([r for r, _ in shapes], np.uint32)
+    cols = np.array([c for _, c in shapes], np.uint32)
+    launch = np.zeros(len(shapes), np.uint32)
+    n = emu().emu_dtw_pack(W, len(shapes), rows.ctypes.data, cols.ctypes.data, budget, launch.ctypes.data)
+    return [int(x) for x in launch], int(n)
+
+
+# (k-mers, kept means) of tests/test_z_gpu_dtw_band.py's long reads (its fixture checks them), and the budget its
+# test_small_budget_skips_only_the_query_over_it gives the aligner: room for every band at W = 64 but the largest
+LONG_READ_SHAPES = [(12546, 19369), (18796, 29123), (28796, 44424), (35046, 54428), (41296, 63875), (49995, 77533),
+                    (2546, 3894), (7546, 11652)]
+
+
+def small_budget(shapes, W):
+    need = sorted(sweep_bytes([s], W) for s in shapes)
+    return (need[-2] + need[-1]) // 2
 
 
 def problem(rng, nr, nc, walk=True, noise=2.5):

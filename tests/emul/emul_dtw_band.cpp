@@ -1,8 +1,9 @@
-// tests/emul/emul_dtw_band.cpp -- the banded DTW sweep (unc_dtw_band.cuh) and, for comparison, k_dtw's routine
-// (unc_dtw.cuh) on the CPU under the warp emulator, one CTA of n_threads fibers taking the problems in turn as the
-// persistent kernels do.  Workspace carved as unc_dtw_batch / unc_dtw_batch_banded carve it.  Test vehicle only.
+// tests/emul/emul_dtw_band.cpp -- the DTW sweeps on the CPU under the warp emulator: the banded sweep (unc_dtw_band.cuh) and
+// k_dtw's full one (unc_dtw.cuh), one CTA of n_threads fibers taking the problems in turn as the persistent kernels do.  The
+// workspace is planned, sized and carved by unc_dtw_plan.hpp, as unc_dtw_batch / unc_dtw_batch_banded plan theirs, in one
+// buffer.  Test vehicle only.
 #include "unc_device.cuh"   // UNC_EMUL is defined on the command line
-#include "unc_dtw_band.cuh"
+#include "unc_dtw_plan.hpp"
 
 #include <vector>
 
@@ -20,54 +21,61 @@ static void full_entry(void *vp) {
 
 extern "C" {
 
-// n problems: means[mean_off[p] .. mean_off[p+1]) against kmers[kmer_off[p] .. kmer_off[p+1]), subseq NONE.  band >= 1:
-// the banded sweep; band 0: k_dtw's full sweep.  Out: path (room for rows + columns pairs at path_off[p]), path_len,
-// score, and (optional) every problem's breadcrumbs one after the other (banded: the in-band cells column-major; full:
-// rows x columns row-major), their total in *n_bc.
-int emu_dtw_sweep(const float *model_means_stdvs, int cost_kind, float dw, float hw, float vw, uint32_t band, uint32_t n,
-                  const float *means, const uint64_t *mean_off, const uint16_t *kmers, const uint64_t *kmer_off,
+// n problems: means[mean_off[p] .. mean_off[p+1]) against kmers[kmer_off[p] .. kmer_off[p+1]).  band >= 1: the banded sweep
+// (subseq 0 only); band 0: k_dtw's full sweep with subseq 0 NONE, 1 ROW or 2 COL.  Out: path (room for rows + columns pairs
+// at path_off[p]), path_len, score, and (optional) every problem's breadcrumbs one after the other (banded: the in-band cells
+// column-major; full: rows x columns row-major), their total in *n_bc.
+int emu_dtw_sweep(const float *model_means_stdvs, int cost_kind, int subseq, float dw, float hw, float vw, uint32_t band,
+                  uint32_t n, const float *means, const uint64_t *mean_off, const uint16_t *kmers, const uint64_t *kmer_off,
                   uint64_t *path, const uint64_t *path_off, uint64_t *path_len, float *score, uint8_t *bc_out,
                   uint64_t *n_bc, int n_threads) {
-    std::vector<float> model(3 * 1024);
-    for (u32 k = 0; k < 1024; k++) {
-        const float mean = model_means_stdvs[2 * k], stdv = model_means_stdvs[2 * k + 1];
-        model[k] = mean;
-        model[1024 + k] = 2 * stdv * stdv;
-        model[2048 + k] = (float) std::log(std::sqrt(M_PI * model[1024 + k]));
-    }
-    std::vector<DevDtwProblem> prob(n);
-    std::vector<u64> col_off;
-    u64 bc_total = 0, diag_total = 0, edge_total = 0;
+    if (band && subseq) return -1;
+    DtwPlan P(band);
     for (u32 i = 0; i < n; i++) {
         const u64 nc = mean_off[i + 1] - mean_off[i], nr = kmer_off[i + 1] - kmer_off[i];
         if (nc == 0 || nr == 0) return -1;
-        DevDtwProblem &P = prob[i];
-        P.mean_off = mean_off[i]; P.kmer_off = kmer_off[i]; P.n_cols = (u32) nc; P.n_rows = (u32) nr;
-        P.bc_off = bc_total; P.diag_off = diag_total; P.edge_off = edge_total; P.path_off = path_off[i];
-        diag_total += UNC_DTW_WORK_FLOATS(nr, nc);
-        if (band) {
-            col_off.resize(edge_total + nc + 1);
-            bc_total += unc_band_offsets(unc_band_make((u32) nr, (u32) nc, band), col_off.data() + edge_total);
-            edge_total += nc + 1;
-        } else {
-            bc_total += nr * nc; edge_total += nr + nc;
-        }
+        P.add((u32) nr, (u32) nc, mean_off[i], kmer_off[i], path_off[i]);
     }
-    // unwritten bytes and floats stay recognisable (a read of one would show up as a wrong result)
-    std::vector<unsigned char> bc(bc_total + 1, 0xEE);
-    std::vector<float> diag(diag_total + 1, -12345.0f), edge(band ? 1 : edge_total + 1, -12345.0f);
-    u32 queue = 0;
+    const std::vector<float> model = dtw_model_table(model_means_stdvs);
+    P.stage(model.data(), means, mean_off[n], kmers, kmer_off[n]);
+    P.t.path = path_off[n];
+    // one buffer as the device workspace: unwritten bytes and floats stay recognisable (a read of one would show up as a
+    // wrong result), and a region the layout undercounts or overlaps corrupts its neighbour
+    const DtwLayout L = dtw_layout(P.t);
+    std::vector<u64> ws(L.bytes / 8);
+    char *w = (char *) ws.data();
+    memset(w, 0xEE, L.bytes);
+    std::fill((float *) (w + L.diag), (float *) (w + L.diag) + P.t.diag, -12345.0f);
+    if (!band) std::fill((float *) (w + L.edge), (float *) (w + L.edge) + P.t.edge, -12345.0f);
     DevDtwBand B;
-    DevDtw &D = B.D;
-    D.model = model.data(); D.means = means; D.kmers = kmers; D.prob = prob.data(); D.n_prob = n;
-    D.bc = bc.data(); D.diag = diag.data(); D.edge = edge.data(); D.path = path; D.path_len = path_len; D.score = score;
-    D.cost_kind = cost_kind; D.subseq = 0; D.dw = dw; D.hw = hw; D.vw = vw; D.queue = &queue;
-    B.col_off = col_off.data(); B.band = band;
+    dtw_carve(P, w, B);
+    memcpy(w + L.model, P.h_model, 3 * 1024 * 4);
+    memcpy(w + L.means, means, P.t.means * 4);
+    memcpy(w + L.kmers, kmers, P.t.kmers * 2);
+    memcpy(w + L.prob, P.prob.data(), P.prob.size() * sizeof(DevDtwProblem));
+    if (band) memcpy(w + L.edge, P.col_off.data(), P.col_off.size() * 8);
+    memset(w + L.queue, 0, 4);
+    B.D.cost_kind = cost_kind; B.D.subseq = subseq; B.D.dw = dw; B.D.hw = hw; B.D.vw = vw;
     SweepArgs a = {&B};
     emu_run_cta(band ? band_entry : full_entry, &a, n_threads > 0 ? n_threads : 64);
-    if (bc_out) memcpy(bc_out, bc.data(), bc_total);
-    if (n_bc) *n_bc = bc_total;
+    memcpy(path_len, w + L.plen, (size_t) n * 8);
+    memcpy(score, w + L.score, (size_t) n * 4);
+    memcpy(path + 2 * path_off[0], B.D.path + 2 * path_off[0], (path_off[n] - path_off[0]) * 16);
+    if (bc_out) memcpy(bc_out, B.D.bc, P.t.bc);
+    if (n_bc) *n_bc = P.t.bc;
     return 0;
+}
+
+// the workspace bytes the span aligner plans for one R x C problem (band 0: the full sweep)
+uint64_t emu_dtw_plan_bytes(uint32_t R, uint32_t C, uint32_t band) {
+    DtwPlan P(band);
+    P.add(R, C, 0, 0, 0);
+    return dtw_layout(P.t).bytes;
+}
+
+// the span aligner's launches (dtw_pack): launch[k] of problem k (rows[k] x cols[k]), 0xFFFFFFFF for a skipped one
+uint32_t emu_dtw_pack(uint32_t band, uint32_t n, const uint32_t *rows, const uint32_t *cols, uint64_t budget, uint32_t *launch) {
+    return dtw_pack(band, n, rows, cols, budget, launch);
 }
 
 // the in-band cells of an R x C problem at half-width band (unc_band_offsets)

@@ -7,7 +7,6 @@
 #include "unc_stream_logic.hpp"
 #include "unc_ordered_logic.hpp"
 #include "unc_selfalign.cuh"
-#include "unc_dtw.cuh"
 #include "unc_selfalign_host.hpp"
 #include "../../include/unc_b200.h"
 #include "unc_host_index.hpp"
@@ -107,41 +106,6 @@ extern "C" int emu_tracker_run(uint32_t min_map_len, float min_mean_conf, float 
     a.clu = clu.data(); a.dir = dir.data(); a.dir_fast = fast.data(); a.max_blocks = max_blocks; a.dir_fast_cap = dir_fast_cap; a.overflow = 0;
     emu_run_warp(trk_entry, &a);
     return (int) a.overflow;      // bit 0: block store overflowed, bit 1: the directory ended in the workspace
-}
-
-// The DTW kernel's per-problem routine (unc_dtw.cuh) under the emulator: one CTA of n_threads fibers per problem.
-struct DtwArgs { const DevDtw *D; };
-static void dtw_entry(void *vp) {
-    const DevDtw *D = ((DtwArgs *) vp)->D;
-    for (u32 pi = 0; pi < D->n_prob; pi++) unc_dtw_problem(*D, pi);
-}
-extern "C" int emu_dtw_batch(const float *model_means_stdvs, int cost_kind, int subseq, float dw, float hw, float vw, uint32_t n_problems,
-                             const float *means, const uint64_t *mean_off, const uint16_t *kmers, const uint64_t *kmer_off,
-                             uint64_t *path, const uint64_t *path_off, uint64_t *path_len, float *score, int n_threads) {
-    std::vector<float> model(3 * 1024);
-    for (uint32_t k = 0; k < 1024; k++) {
-        const float mean = model_means_stdvs[2 * k], stdv = model_means_stdvs[2 * k + 1];
-        model[k] = mean; model[1024 + k] = 2 * stdv * stdv; model[2048 + k] = (float) std::log(std::sqrt(M_PI * model[1024 + k]));
-    }
-    std::vector<DevDtwProblem> prob(n_problems);
-    uint64_t bc_total = 0, diag_total = 0, edge_total = 0;
-    for (uint32_t i = 0; i < n_problems; i++) {
-        const uint64_t nc = mean_off[i + 1] - mean_off[i], nr = kmer_off[i + 1] - kmer_off[i];
-        DevDtwProblem &P = prob[i];
-        P.mean_off = mean_off[i]; P.kmer_off = kmer_off[i]; P.n_cols = (u32) nc; P.n_rows = (u32) nr;
-        P.bc_off = bc_total; P.diag_off = diag_total; P.edge_off = edge_total; P.path_off = path_off[i];
-        bc_total += nr * nc; diag_total += UNC_DTW_WORK_FLOATS(nr, nc); edge_total += nr + nc;
-    }
-    std::vector<unsigned char> bc(bc_total + 1);
-    std::vector<float> diag(diag_total + 1), edge(edge_total + 1);
-    u32 queue = 0;
-    DevDtw D;
-    D.model = model.data(); D.means = means; D.kmers = kmers; D.prob = prob.data(); D.n_prob = n_problems;
-    D.bc = bc.data(); D.diag = diag.data(); D.edge = edge.data(); D.path = path; D.path_len = path_len; D.score = score;
-    D.cost_kind = cost_kind; D.subseq = subseq; D.dw = dw; D.hw = hw; D.vw = vw; D.queue = &queue;
-    DtwArgs a = {&D};
-    emu_run_cta(dtw_entry, &a, n_threads > 0 ? n_threads : 64);
-    return 0;
 }
 
 // The mapper's per-event trace in the oracle's row layout (orc_trace_row / orc_trace_seed of oracle/unc_oracle.h), so

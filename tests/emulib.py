@@ -65,7 +65,7 @@ def build():
     out = os.path.join(EMUL_DIR, "libunc_emul.so")
     deps = [src, os.path.join(EMUL_DIR, "warp_emul.hpp")] + \
            [os.path.join(ROOT, "uncalled_b200", "csrc", f) for f in
-            ("unc_device.cuh", "unc_k2v2.cuh", "unc_dtw.cuh", "unc_k1.cuh", "unc_stream.cuh", "unc_stream_logic.hpp", "unc_ordered_logic.hpp", "unc_pdqsort.cuh", "unc_warp.cuh", "unc_host_index.hpp", "unc_host_params.hpp",
+            ("unc_device.cuh", "unc_k2v2.cuh", "unc_k1.cuh", "unc_stream.cuh", "unc_stream_logic.hpp", "unc_ordered_logic.hpp", "unc_pdqsort.cuh", "unc_warp.cuh", "unc_host_index.hpp", "unc_host_params.hpp",
              "unc_selfalign.cuh", "unc_selfalign_host.hpp")]
     if os.path.exists(out) and all(os.path.getmtime(out) >= os.path.getmtime(d) for d in deps):
         return out

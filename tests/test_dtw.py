@@ -6,7 +6,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import emulib
+import dtwbandlib
 import orclib
 
 u64p = C.POINTER(C.c_uint64)
@@ -74,19 +74,7 @@ def test_oracle_dtw_equals_the_reference_classes():
 
 
 def _emul(kind, sub, w, probs, n_threads):
-    L = emulib.lib()
-    L.emu_dtw_batch.argtypes = [f32p, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_uint32, f32p, u64p, u16p, u64p, u64p, u64p, u64p,
-                                f32p, C.c_int]
-    n = len(probs)
-    moff = np.zeros(n + 1, np.uint64); koff = np.zeros(n + 1, np.uint64); poff = np.zeros(n + 1, np.uint64)
-    moff[1:] = np.cumsum([len(m) for m, _ in probs]); koff[1:] = np.cumsum([len(k) for _, k in probs])
-    poff[1:] = np.cumsum([len(m) + len(k) for m, k in probs])
-    am = np.concatenate([m for m, _ in probs]); ak = np.concatenate([k for _, k in probs])
-    path = np.zeros(2 * int(poff[-1]), np.uint64); plen = np.zeros(n, np.uint64); score = np.zeros(n, np.float32)
-    assert L.emu_dtw_batch(TAB.ctypes.data_as(f32p), kind, sub, w[0], w[1], w[2], n, am.ctypes.data_as(f32p), moff.ctypes.data_as(u64p),
-                           ak.ctypes.data_as(u16p), koff.ctypes.data_as(u64p), path.ctypes.data_as(u64p), poff.ctypes.data_as(u64p),
-                           plen.ctypes.data_as(u64p), score.ctypes.data_as(f32p), n_threads) == 0
-    return [(path[2 * int(poff[i]):2 * (int(poff[i]) + int(plen[i]))].reshape(-1, 2), float(score[i])) for i in range(n)]
+    return [(path, score) for path, score, _ in dtwbandlib.emulated(probs, 0, kind, w, n_threads=n_threads, subseq=sub)]
 
 
 @pytest.mark.parametrize("kind", [0, 1])

@@ -189,6 +189,43 @@ def test_emulated_kernel_on_long_reads():
         assert path[0, 0] == len(means) - 1 and path[0, 1] == len(km) - 1 and not path[-1].any()
 
 
+# ---------------------------------------------------------------- the workspace plan (unc_dtw_plan.hpp)
+
+def test_workspace_plan_bytes_and_packing():
+    """the plan's byte count equals the restatement (dtwbandlib.sweep_bytes) over shapes at 1 x 1, R = 1, C = 1, tile edges
+    and W >= R - 1, for both sweeps; the aligner's packing keeps query order, closes a launch only when the next query
+    would pass the budget, keeps every launch within it, skips exactly the queries over it on their own and puts every
+    other query in one launch"""
+    sizes = [1, 2, 7, 8, 9, 15, 16, 17, 63, 64, 65, 200]
+    shapes = [(r, c) for r in sizes for c in sizes] + [(r, c) for r, c, _ in B.SHAPES]
+    for W in (0, 1, 3, 8, 64, 250):
+        for R, C_ in shapes:
+            assert int(B.emu().emu_dtw_plan_bytes(R, C_, W)) == B.sweep_bytes([(R, C_)], W), (R, C_, W)
+
+    def check(shapes, W, budget):
+        launch, n = B.pack(shapes, W, budget)
+        alone = [B.sweep_bytes([s], W) for s in shapes]
+        assert [k for k in range(len(shapes)) if launch[k] == B.SKIP] == [k for k in range(len(shapes)) if alone[k] > budget]
+        kept = [(k, l) for k, l in enumerate(launch) if l != B.SKIP]
+        assert [l for _, l in kept] == sorted(l for _, l in kept) and {l for _, l in kept} == set(range(n))
+        for l in range(n):
+            ks = [k for k, x in kept if x == l]
+            assert B.sweep_bytes([shapes[k] for k in ks], W) <= budget, (l, ks)
+            if l + 1 < n:                              # closed because the next query (maybe one skipped) did not fit
+                assert B.sweep_bytes([shapes[k] for k in ks + [ks[-1] + 1]], W) > budget, (l, ks)
+        return launch, n
+
+    rng = np.random.default_rng(12)
+    for trial in range(40):
+        shapes = [(int(rng.integers(1, 3000)), int(rng.integers(1, 3000))) for _ in range(int(rng.integers(1, 30)))]
+        W = int(rng.choice([0, 1, 8, 64]))
+        alone = sorted(B.sweep_bytes([s], W) for s in shapes)
+        budget = int(rng.choice([alone[0] - 1, alone[len(alone) // 2], alone[-1], 3 * alone[-1], 100 * alone[-1]]))
+        check(shapes, W, budget)
+    launch, n = check(B.LONG_READ_SHAPES, 64, B.small_budget(B.LONG_READ_SHAPES, 64))
+    assert launch.count(B.SKIP) == 1 and n >= 2
+
+
 # ---------------------------------------------------------------- argument checks
 
 def test_restatement_rejects_what_the_band_does_not_define():

@@ -90,6 +90,7 @@ def long_reads(tmp_path_factory):
         cases.append(("r%d" % i, sig, contig, st, st + ln, fwd))
     recs = [DA.oracle_align(g, *c[1:]) for c in cases]
     assert sum(r["status"] == 1 for r in recs) >= 3
+    assert [(len(r["_kmers"]), len(r["_means"])) for r in recs] == B.LONG_READ_SHAPES
     return prefix, cases, recs
 
 
@@ -121,21 +122,12 @@ def test_aligner_band_aligns_long_reads(long_reads, W):
     assert cells == want_cells and launches >= 1
 
 
-def _sweep_bytes(R, C_, W):
-    """the aligner's workspace for one banded problem (SweepNeed::bytes in unc_dtw_align_host.inl): problem record,
-    in-band breadcrumbs, hrow / vcol / corners, column offsets, path room, path length, score, queue; 256-byte aligned"""
-    a = lambda x: (x + 255) // 256 * 256
-    lo, hi = B.band_rows(R, C_, W)
-    return a(56) + a(int((hi - lo + 1).sum())) + a(4 * (C_ + R + 3 * ((R + 7) // 8) + 8)) + a(8 * (C_ + 1)) + a(16 * (R + C_)) + \
-        a(8) + a(4) + a(4)
-
-
 def test_small_budget_skips_only_the_query_over_it(long_reads):
     prefix, cases, recs = long_reads
     W = 64
-    need = [_sweep_bytes(len(r["_kmers"]), len(r["_means"]), W) for r in recs]
-    big = int(np.argmax(need))
-    budget = (sorted(need)[-2] + need[big]) // 2                    # room for every band but the largest
+    shapes = [(len(r["_kmers"]), len(r["_means"])) for r in recs]
+    big = int(np.argmax([B.sweep_bytes([s], W) for s in shapes]))
+    budget = B.small_budget(shapes, W)                               # room for every band but the largest
     got, (_, launches, _) = _align(prefix, cases, W, budget=budget)
     full, _ = _align(prefix, cases, W)
     for i, (g, f) in enumerate(zip(got, full)):

@@ -107,7 +107,7 @@ def build(force=False, verbose=False):
     src_dir = os.path.join(PKG_DIR, "csrc")
     srcs = [os.path.join(src_dir, f) for f in ("unc_abi.cu", "unc_index_build.cpp", "unc_fast5.cpp")]
     deps = srcs + [os.path.join(src_dir, f) for f in
-                   ("unc_device.cuh", "unc_k2v2.cuh", "unc_dtw.cuh", "unc_dtw_band.cuh", "unc_dtw_host.inl", "unc_dtw_align.cuh", "unc_dtw_align_host.inl", "unc_k1.cuh", "unc_stream.cuh", "unc_stream_host.inl", "unc_stream_logic.hpp", "unc_replay.cuh", "unc_replay_host.inl", "unc_events.cuh", "unc_events_host.inl", "unc_ordered_logic.hpp", "unc_pdqsort.cuh", "unc_warp.cuh",
+                   ("unc_device.cuh", "unc_k2v2.cuh", "unc_dtw.cuh", "unc_dtw_band.cuh", "unc_dtw_plan.hpp", "unc_dtw_host.inl", "unc_dtw_align.cuh", "unc_dtw_align_host.inl", "unc_k1.cuh", "unc_stream.cuh", "unc_stream_host.inl", "unc_stream_logic.hpp", "unc_replay.cuh", "unc_replay_host.inl", "unc_events.cuh", "unc_events_host.inl", "unc_ordered_logic.hpp", "unc_pdqsort.cuh", "unc_warp.cuh",
                     "unc_selfalign.cuh", "unc_selfalign_host.hpp", "unc_selfalign_host.inl",
                     "unc_mask.cuh", "unc_mask_host.hpp", "unc_mask_host.inl",
                     "unc_mask_ext.cuh", "unc_mask_ext_host.hpp", "unc_mask_ext_host.inl",
