@@ -115,7 +115,8 @@ typedef struct {
     uint64_t n_rows;  /* FM-index length (fwd + revcomp) */
     int32_t n_seqs;
     int32_t device;
-    uint64_t device_bytes;
+    uint64_t device_bytes;  /* the index's device tables; 4 (n_rows + 1) of them are the expanded suffix array when
+                               the load built it */
     uint32_t n_kmer_groups;
 } unc_index_info;
 
@@ -225,7 +226,17 @@ int unc_events_batch(unc_pool *pool, const unc_read_desc *reads, uint32_t n_read
 /* pore-model log-probabilities of one normalised event against all 1024 k-mers, computed
  * on the device with the mapper's own routine (parity probe). */
 int unc_match_probs(const unc_index *idx, float event, float out[1024]);
-/* FM probes computed on the device (parity probes): one backward step per entry, and SA. */
+/* FM probes computed on the device by the mapper's own routines (parity probes).
+ *   unc_fm_step       the mapper's backward step, per entry i: rows start[i]-1 and end[i] (1 <= start <= n_rows + 1,
+ *                     end <= n_rows); ns[4i+c] = L2[c] + Occ(start-1, c) + 1 and ne[4i+c] = L2[c] + Occ(end, c) for
+ *                     all four bases, and valid[i] bit c set iff bit c of want[i] is and ns <= ne.
+ *   unc_fm_neighbors  the same step for one base per entry (BwaIndex::get_neighbor): an empty range reads
+ *                     start = end + 1 as there.
+ *   unc_fm_sa         bwt_sa at rows 0..n_rows as the mapper reads it: from the expanded suffix array when the index
+ *                     load built one (it does not when device memory is short or UNC_NO_SA_EXPAND is set), by the LF
+ *                     walk over the sampled array otherwise. */
+int unc_fm_step(const unc_index *idx, uint32_t n, const uint64_t *start, const uint64_t *end, const uint8_t *want,
+                uint64_t *ns, uint64_t *ne, uint8_t *valid);
 int unc_fm_neighbors(const unc_index *idx, uint32_t n, const uint64_t *start, const uint64_t *end,
                      const uint8_t *base, uint64_t *ostart, uint64_t *oend);
 int unc_fm_sa(const unc_index *idx, uint32_t n, const uint64_t *rows, uint64_t *out);

@@ -296,6 +296,17 @@ uint64_t emu_sa(void *pidx, uint64_t row) {
     return unc_sa(e->ix, (u32) row, &a, &b);
 }
 
+// unc_fm_step of unc_abi.cu on the emulator's occ2 blocks: ns / ne hold 4 entries per query
+void emu_fm_step(void *pidx, uint32_t n, const uint64_t *st, const uint64_t *en, const uint8_t *want, uint64_t *ns,
+                 uint64_t *ne, uint8_t *valid) {
+    EmuIndex *e = (EmuIndex *) pidx;
+    for (uint32_t i = 0; i < n; i++) {
+        u32 s[4], t[4], nb = 0;
+        valid[i] = (uint8_t) unc_occ2_neighbors(e->ix, (u32) st[i], (u32) en[i], want[i], s, t, &nb);
+        for (u32 b = 0; b < 4; b++) { ns[(size_t) i * 4 + b] = s[b]; ne[(size_t) i * 4 + b] = t[b]; }
+    }
+}
+
 
 // ---------------------------------------------------------------- streaming path under the emulator
 struct EmuStream {

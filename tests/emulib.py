@@ -119,6 +119,8 @@ def _bind(L):
     L.emu_free.restype = None
     L.emu_sa.argtypes = [C.c_void_p, C.c_uint64]
     L.emu_sa.restype = C.c_uint64
+    L.emu_fm_step.argtypes = [C.c_void_p, C.c_uint32] + [C.c_void_p] * 6
+    L.emu_fm_step.restype = None
     L.emu_k1_stats.argtypes = [C.c_void_p]
     L.emu_stream_create.restype = C.c_void_p
     L.emu_stream_create.argtypes = [C.c_void_p, C.POINTER(UncParams), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
@@ -169,6 +171,27 @@ class Emu:
             raise RuntimeError("emu_map_batch rc=%d" % rc)
         return list(out), [ev[i, :ne[i]].copy() for i in range(n)], [nm[i, :ne[i]].copy() for i in range(n)], mel
 
+
+    def fm_step(self, start, end, want):
+        """unc_fm_step on the emulator: (ns, ne) of shape (n, 4) and the valid masks, as uncalled_b200.Index.fm_step."""
+        start = np.ascontiguousarray(start, np.uint64)
+        end = np.ascontiguousarray(end, np.uint64)
+        want = np.ascontiguousarray(want, np.uint8)
+        ns, ne, valid = np.zeros((len(start), 4), np.uint64), np.zeros((len(start), 4), np.uint64), np.zeros_like(want)
+        self.L.emu_fm_step(self.idx, len(start), start.ctypes.data, end.ctypes.data, want.ctypes.data, ns.ctypes.data,
+                           ne.ctypes.data, valid.ctypes.data)
+        return ns, ne, valid
+
+    def sa(self, rows):
+        return np.array([self.L.emu_sa(self.idx, int(r)) for r in rows], np.uint64)
+
+    def kmer_ranges(self):
+        st, en = np.zeros(1024, np.uint64), np.zeros(1024, np.uint64)
+        a, b = C.c_uint64(), C.c_uint64()
+        for k in range(1024):
+            self.L.emu_kmer_range(self.idx, k, C.byref(a), C.byref(b))
+            st[k], en[k] = a.value, b.value
+        return st, en
 
     def set_tie_order(self, mode):
         """1: the exact-ties kernel (the reference's pdqsort reproduced), 0: the default kernel."""

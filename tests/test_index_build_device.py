@@ -8,7 +8,8 @@ come before anything is written; the bindings keep the host builder without a de
 
 GPU tier: the same inputs and seeded genomes of 1 Mb and 60 Mb (above bwa's `bwtsw` switch) against the host builder,
 `uncalled index` end to end, and a 1.1 Gbp genome (2.2e9 FM rows, above 2^31) against the digests of bwa's own files,
-loaded and searched and mapped against."""
+loaded and searched and mapped against, its backward step probed around 2^31, primary and the last rows, and its SA read
+from the expanded table and by the LF walk."""
 import hashlib
 import json
 import os
@@ -260,8 +261,53 @@ def test_gpu_above_2_31_rows_against_bwa(tmp_path):
         l_pac = int(open(prefix + ".ann").readline().split()[0])
         n = 2 * l_pac
         assert idx.n_rows == n and n + 1 > 2 ** 31
-        fwd = _pac_codes(prefix, l_pac)
         rng = np.random.default_rng(5)
+
+        # the mapper's backward step (unc_fm_step) against bwt_occ restated per row from the .bwt file: every row within
+        # 200 of 2^31 and of primary, the last 300 rows, 5000 random rows, each as start - 1 and as end
+        import fmsteplib as F
+        primary = int(np.fromfile(prefix + ".bwt", np.uint64, 1)[0])
+        rows = np.unique(np.concatenate([np.arange(2 ** 31 - 200, 2 ** 31 + 201), np.arange(primary - 200, primary + 201),
+                                         np.arange(n - 299, n + 1), rng.integers(0, n + 1, 5000)]))
+        rows = rows[(rows >= 0) & (rows <= n)]
+        st, en = F.pairs_at_rows(rows, n, rng)
+        want = rng.integers(0, 16, len(st)).astype(np.uint8)
+        ns, ne, valid = idx.fm_step(st, en, want)
+        xs, xe = F.step_at_rows(prefix, st, en)
+        assert np.array_equal(ns.astype(np.int64), xs) and np.array_equal(ne.astype(np.int64), xe)
+        xv = ((((want[:, None].astype(np.int64) >> np.arange(4)) & 1) == 1) & (xs <= xe)) @ (1 << np.arange(4))
+        assert np.array_equal(valid.astype(np.int64), xv)
+        print("1.1 Gbp step: %d queries at %d rows, primary %d" % (len(st), len(rows), primary))
+
+        # the SA as the mapper reads it, against a second load that walks LF, when the device has room for one
+        import torch
+        free_b, _ = torch.cuda.mem_get_info(0)
+        need = idx.device_bytes + (1 << 30)
+        if free_b > need:
+            with_walk = os.environ.get("UNC_NO_SA_EXPAND")
+            os.environ["UNC_NO_SA_EXPAND"] = "1"
+            try:
+                walk = U.Index(prefix, device=0)
+            finally:
+                if with_walk is None:
+                    del os.environ["UNC_NO_SA_EXPAND"]
+                else:
+                    os.environ["UNC_NO_SA_EXPAND"] = with_walk
+            try:
+                diff = idx.device_bytes - walk.device_bytes
+                assert diff in (0, 4 * (n + 1)), diff
+                print("1.1 Gbp SA: first load %s, second load walks LF" %
+                      ("read the expanded suffix array" if diff else "walked LF too (device memory short)"))
+                sa_rows = np.unique(np.concatenate([np.arange(2 ** 31 - 300, 2 ** 31 + 301), rng.integers(1, n + 1, 3000),
+                                                    np.arange(primary - 100, primary + 101), np.arange(n - 100, n + 1)]))
+                sa_rows = sa_rows[(sa_rows >= 1) & (sa_rows <= n)].astype(np.uint64)
+                assert np.array_equal(idx.sa(sa_rows), walk.sa(sa_rows))
+            finally:
+                walk.close()
+        else:
+            print("1.1 Gbp SA: second load (LF walk) skipped, %d bytes free, %d needed" % (free_b, need))
+
+        fwd = _pac_codes(prefix, l_pac)
 
         # suffix order of consecutive rows, read from the text (forward codes, then their reverse complement)
         def sym(pos):                          # text symbols at positions pos (array), 4 past the end

@@ -89,7 +89,7 @@ class Fast5Read(C.Structure):
 EXPORTS = ["unc_strerror", "unc_last_error", "unc_device_count", "unc_init", "unc_shutdown", "unc_params_default",
            "unc_index_load", "unc_index_get_info", "unc_index_seq", "unc_index_kmer_range",
            "unc_index_thresholds", "unc_index_free", "unc_index_build", "unc_pool_create", "unc_pool_free",
-           "unc_map_batch", "unc_map_batch_device", "unc_map_batch_ordered", "unc_pool_set_tie_order", "unc_map_batch_submit", "unc_map_batch_wait", "unc_pool_record", "unc_pool_elapsed", "unc_events_batch", "unc_match_probs", "unc_fm_neighbors",
+           "unc_map_batch", "unc_map_batch_device", "unc_map_batch_ordered", "unc_pool_set_tie_order", "unc_map_batch_submit", "unc_map_batch_wait", "unc_pool_record", "unc_pool_elapsed", "unc_events_batch", "unc_match_probs", "unc_fm_step", "unc_fm_neighbors",
            "unc_fm_sa", "unc_pool_last_timing", "unc_pool_k1_stats", "unc_stream_create", "unc_stream_set_tie_order", "unc_stream_set_chunk_timeout", "unc_stream_last_step_ms", "unc_stream_channel_norm", "unc_stream_step", "unc_stream_replay",
            "unc_stream_free", "unc_self_align", "unc_free", "unc_fast5_open", "unc_fast5_count", "unc_fast5_info",
            "unc_fast5_load", "unc_fast5_close", "unc_fast5_last_error", "unc_dtw_batch", "unc_dtw_release", "unc_dtw_last_kernel_ms",
@@ -187,6 +187,7 @@ def lib():
     L.unc_pool_elapsed.argtypes = [vp, C.c_int, vp, C.c_int, C.POINTER(C.c_float)]
     L.unc_events_batch.argtypes = [vp, vp, u32, vp, u32, vp, vp, vp, vp]
     L.unc_match_probs.argtypes = [vp, C.c_float, vp]
+    L.unc_fm_step.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp]
     L.unc_fm_neighbors.argtypes = [vp, u32, vp, vp, vp, vp, vp]
     L.unc_fm_sa.argtypes = [vp, u32, vp, vp]
     L.unc_pool_last_timing.argtypes = [vp, C.POINTER(Timing)]

@@ -126,26 +126,21 @@ __global__ void k_match_probs(DevIndex ix, float event, float *out) {
     if (k < UNC_NKMER) out[k] = unc_match_prob(event, ix.lv_mean[k], ix.lv_var2[k], ix.lognorm[k]);
 }
 
-__global__ void k_fm_neighbors(DevIndex ix, u32 n, const u64 *st, const u64 *en, const u8 *base, u64 *ost, u64 *oen) {
+// the mapper's backward step (unc_occ2_neighbors) per entry: four (start, end) pairs and the valid mask
+__global__ void k_fm_step(DevIndex ix, u32 n, const u64 *st, const u64 *en, const u8 *want, u64 *ons, u64 *one, u8 *valid) {
     u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    u32 ns[4], ne[4], nb = 0, c = base[i];
-    u32 ok = unc_neighbors(ix, (u32) st[i], (u32) en[i], 1u << c, ns, ne, &nb);
-    if (!((ok >> c) & 1u)) {   // empty range: report it the way get_neighbor does (start = end + 1 ...)
-        ns[c] = unc_L2(ix, c) + unc_occ(ix, (u32) st[i] - 1u, c, &nb) + 1u;
-        ne[c] = unc_L2(ix, c) + unc_occ(ix, (u32) en[i], c, &nb);
-    }
-    ost[i] = ns[c];
-    oen[i] = ne[c];
+    u32 ns[4], ne[4], nb = 0;
+    valid[i] = (u8) unc_occ2_neighbors(ix, (u32) st[i], (u32) en[i], want[i], ns, ne, &nb);
+    for (u32 b = 0; b < 4; b++) { ons[(size_t) i * 4 + b] = ns[b]; one[(size_t) i * 4 + b] = ne[b]; }
 }
 
+// bwt_sa as the mapper reads it: the expanded table when the index load built one, the LF walk otherwise
 __global__ void k_fm_sa(DevIndex ix, u32 n, const u64 *rows, u64 *out) {
     u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     u32 a = 0, b = 0;
-    // widen like the reference: sa[0] = (u64)-1
-    u32 v = unc_sa(ix, (u32) rows[i], &a, &b);
-    out[i] = v;
+    out[i] = unc_sa_lookup(ix, (u32) rows[i], &a, &b);
 }
 
 // ------------------------------------------------------------------ host state
@@ -889,25 +884,45 @@ int unc_match_probs(const unc_index *x, float event, float out[1024]) {
     return UNC_OK;
 }
 
+int unc_fm_step(const unc_index *x, uint32_t n, const uint64_t *start, const uint64_t *end, const uint8_t *want,
+                uint64_t *ns, uint64_t *ne, uint8_t *valid) {
+    if (!x || !n || !start || !end || !want || !ns || !ne || !valid) return fail(UNC_E_ARG, "null argument");
+    for (uint32_t i = 0; i < n; i++)   // the step reads the Occ blocks of rows start-1 and end, both in [0, seq_len]
+        if (start[i] < 1 || start[i] > x->h.seq_len + 1 || end[i] > x->h.seq_len) return fail(UNC_E_ARG, "row out of range");
+    CUDA_TRY(cudaSetDevice(x->device));
+    DevMem<u64> ds, de, dns, dne;
+    DevMem<u8> dw, dv;
+    int rc;
+    if ((rc = ds.upload(start, (size_t) n * 8, 0, "start rows")) || (rc = de.upload(end, (size_t) n * 8, 0, "end rows")) ||
+        (rc = dw.upload(want, n, 0, "wanted bases")) || (rc = dns.alloc((size_t) n * 4, "neighbour start rows")) ||
+        (rc = dne.alloc((size_t) n * 4, "neighbour end rows")) || (rc = dv.alloc(n, "valid masks")))
+        return rc;
+    k_fm_step<<<(n + 127) / 128, 128>>>(x->ix, n, ds, de, dw, dns, dne, dv);
+    CUDA_TRY(cudaMemcpy(ns, dns, (size_t) n * 32, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(ne, dne, (size_t) n * 32, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(valid, dv, n, cudaMemcpyDeviceToHost));
+    return UNC_OK;
+}
+
 int unc_fm_neighbors(const unc_index *x, uint32_t n, const uint64_t *start, const uint64_t *end, const uint8_t *base,
                      uint64_t *ostart, uint64_t *oend) {
-    if (!x || !n) return fail(UNC_E_ARG, "null argument");
-    CUDA_TRY(cudaSetDevice(x->device));
-    DevMem<u64> ds, de, dos, doe;
-    DevMem<u8> db;
-    int rc;
-    if ((rc = ds.upload(start, n * 8, 0, "start rows")) || (rc = de.upload(end, n * 8, 0, "end rows")) ||
-        (rc = db.upload(base, n, 0, "bases")) || (rc = dos.alloc(n, "neighbour start rows")) ||
-        (rc = doe.alloc(n, "neighbour end rows")))
-        return rc;
-    k_fm_neighbors<<<(n + 127) / 128, 128>>>(x->ix, n, ds, de, db, dos, doe);
-    CUDA_TRY(cudaMemcpy(ostart, dos, n * 8, cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(oend, doe, n * 8, cudaMemcpyDeviceToHost));
+    if (!x || !n || !base || !ostart || !oend) return fail(UNC_E_ARG, "null argument");
+    std::vector<uint8_t> want(n), valid(n);
+    std::vector<uint64_t> ns((size_t) n * 4), ne((size_t) n * 4);
+    for (uint32_t i = 0; i < n; i++) {
+        if (base[i] > 3) return fail(UNC_E_ARG, "base out of range");
+        want[i] = (uint8_t) (1u << base[i]);
+    }
+    if (int rc = unc_fm_step(x, n, start, end, want.data(), ns.data(), ne.data(), valid.data())) return rc;
+    // every base's range is computed, so an empty one reads as get_neighbor reports it (start = end + 1 ...)
+    for (uint32_t i = 0; i < n; i++) { ostart[i] = ns[(size_t) i * 4 + base[i]]; oend[i] = ne[(size_t) i * 4 + base[i]]; }
     return UNC_OK;
 }
 
 int unc_fm_sa(const unc_index *x, uint32_t n, const uint64_t *rows, uint64_t *out) {
-    if (!x || !n) return fail(UNC_E_ARG, "null argument");
+    if (!x || !n || !rows || !out) return fail(UNC_E_ARG, "null argument");
+    for (uint32_t i = 0; i < n; i++)
+        if (rows[i] > x->h.seq_len) return fail(UNC_E_ARG, "row out of range");
     CUDA_TRY(cudaSetDevice(x->device));
     DevMem<u64> dr, dout;
     int rc;

@@ -209,57 +209,6 @@ UNC_DEV u32 unc_occ(const DevIndex &ix, u32 k, u32 c, u32 *n_blocks) {
     return unc_occ_in_block(b.b0, b.b1, b.b2, b.b3, kk, c);
 }
 
-// One backward-search step for all four bases at once: BwaIndex::get_neighbor
-// (reference src/bwa_index.hpp:158-162) over bwt_2occ (submods/bwa/bwt.c:132-163).
-// `want` has bit b set for each base whose range is needed; on return bit b of the result is
-// set iff base b yields a valid (non-empty) range, stored in ns[b]..ne[b].
-// Paths always have start >= 1.  Instead of two Occ values per base, the symbols of rows
-// (k, l] are counted first: only bases that occur there have a non-empty range (for a
-// unique path that is exactly one base), and only for those the prefix Occ(k, c) is needed:
-//   ns = L2[c] + Occ(k,c) + 1,  ne = L2[c] + Occ(l,c) = ns + count_c(k,l] - 1.
-// `pre` (optional): the Occ block of row start-1, already fetched (staged by cp.async in the extension loop)
-UNC_DEV u32 unc_neighbors(const DevIndex &ix, u32 start, u32 end, u32 want, u32 ns[4], u32 ne[4], u32 *n_blocks,
-                          const OccBlock *pre = nullptr) {
-    u32 k = start - 1, l = end;
-    u32 kk = k - (k >= ix.primary), ll = l - (l >= ix.primary);
-    bool l_is_end = (l == ix.seq_len);
-    OccBlock bk = pre ? *pre : unc_load_block(ix, kk);
-    (*n_blocks)++;
-    u32 valid = 0;
-    if (!l_is_end && (ll >> 5) == (kk >> 5)) {
-        // rows k and l fall into the same 64-bit BWT word: count symbols of (kk, ll] directly
-        u32 q = (kk & 127u) >> 5;
-        u32 hi = q == 0 ? bk.b2.x : q == 1 ? bk.b2.z : q == 2 ? bk.b3.x : bk.b3.z;
-        u32 lo = q == 0 ? bk.b2.y : q == 1 ? bk.b2.w : q == 2 ? bk.b3.y : bk.b3.w;
-        u64 w = ((u64) hi << 32) | lo;
-        u64 le_k = ~((1ull << ((~kk & 31u) << 1)) - 1ull), le_l = ~((1ull << ((~ll & 31u) << 1)) - 1ull);
-        u64 between = le_l & ~le_k;
-#pragma unroll
-        for (u32 c = 0; c < 4; c++) {
-            if (!((want >> c) & 1u)) continue;
-            u32 cnt = (u32) d_popcll(unc_match_bits(w, c) & between);
-            if (cnt == 0) continue;
-            u32 ok = unc_occ_in_block(bk.b0, bk.b1, bk.b2, bk.b3, kk, c);
-            ns[c] = unc_L2(ix, c) + ok + 1;
-            ne[c] = ns[c] + cnt - 1;
-            valid |= 1u << c;
-        }
-        return valid;
-    }
-    OccBlock bl = bk;
-    if (!l_is_end && (ll >> 7) != (kk >> 7)) { bl = unc_load_block(ix, ll); (*n_blocks)++; }
-#pragma unroll
-    for (u32 c = 0; c < 4; c++) {
-        if (!((want >> c) & 1u)) continue;
-        u32 ok = unc_occ_in_block(bk.b0, bk.b1, bk.b2, bk.b3, kk, c);
-        u32 ol = l_is_end ? (unc_L2(ix, c + 1) - unc_L2(ix, c)) : unc_occ_in_block(bl.b0, bl.b1, bl.b2, bl.b3, ll, c);
-        ns[c] = unc_L2(ix, c) + ok + 1;
-        ne[c] = unc_L2(ix, c) + ol;
-        if (ns[c] <= ne[c]) valid |= 1u << c;
-    }
-    return valid;
-}
-
 // bwt_sa (reference submods/bwa/bwt.c:86-96) with bwt_invPsi (:53-59); sa_intv == 32
 UNC_DEV u32 unc_sa(const DevIndex &ix, u32 k, u32 *n_steps, u32 *n_blocks) {
     u32 steps = 0;

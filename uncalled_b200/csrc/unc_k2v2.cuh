@@ -62,6 +62,48 @@ UNC_DEV void unc_occ2_all(const uint4 cnt, const uint4 sym, u32 p, u32 o[4]) {
     o[0] = cnt.x + (p + 1u - c1 - c2 - c3); o[1] = cnt.y + c1; o[2] = cnt.z + c2; o[3] = cnt.w + c3;
 }
 
+// One backward-search step for all four bases: BwaIndex::get_neighbor (reference src/bwa_index.hpp:158-162) over
+// bwt_2occ (submods/bwa/bwt.c:132-163).  For each base b in order, with nsb = L2[b] + Occ(ST-1, b) + 1 and
+// neb = L2[b] + Occ(EN, b), wanted or not, and vb = (bit b of WANT is set and nsb <= neb), runs the statements passed
+// after BLOCKS; BLOCKS grows by the reference's 128-row blocks the step reads.  ST >= 1 (paths and k-mer ranges never
+// start at row 0).  A macro rather than a function so that the worker warps (unc_k2_workers_v2) and unc_occ2_neighbors
+// expand the same body in place: called as a function, it changes how ptxas allocates the map kernels' registers.
+#define UNC_OCC2_STEP(IX, ST, EN, WANT, BLOCKS, ...)                                                                       \
+    do {                                                                                                               \
+        const u32 k0_ = (ST) - 1u, l0_ = (EN);                                                                         \
+        const u32 kk_ = k0_ - (k0_ >= (IX).primary), ll_ = l0_ - (l0_ >= (IX).primary);                                \
+        const bool l_is_end_ = (l0_ == (IX).seq_len);                                                                  \
+        const uint4 *bk_ = (IX).occ2 + ((size_t) (kk_ >> 6) << 1);                                                     \
+        const uint4 kc_ = d_ldg(bk_), ks_ = d_ldg(bk_ + 1);                                                            \
+        uint4 lc_ = kc_, ls_ = ks_;                                                                                    \
+        if (!l_is_end_ && (ll_ >> 6) != (kk_ >> 6)) {                                                                  \
+            const uint4 *bl_ = (IX).occ2 + ((size_t) (ll_ >> 6) << 1);                                                 \
+            lc_ = d_ldg(bl_); ls_ = d_ldg(bl_ + 1);                                                                    \
+        }                                                                                                              \
+        BLOCKS += 1u + ((!l_is_end_ && (ll_ >> 7) != (kk_ >> 7)) ? 1u : 0u);                                           \
+        u32 ok_[4], ol_[4];                                                                                            \
+        unc_occ2_all(kc_, ks_, kk_ & 63u, ok_);                                                                        \
+        unc_occ2_all(lc_, ls_, ll_ & 63u, ol_);                                                                        \
+        if (l_is_end_) {                                                                                               \
+            ol_[0] = (IX).L2[1] - (IX).L2[0]; ol_[1] = (IX).L2[2] - (IX).L2[1];                                        \
+            ol_[2] = (IX).L2[3] - (IX).L2[2]; ol_[3] = (IX).L2[4] - (IX).L2[3];                                        \
+        }                                                                                                              \
+        _Pragma("unroll")                                                                                              \
+        for (u32 b = 0; b < 4; b++) {                                                                                  \
+            const u32 nsb = (IX).L2[b] + ok_[b] + 1u, neb = (IX).L2[b] + ol_[b];                                       \
+            const bool vb = (((WANT) >> b) & 1u) && nsb <= neb;                                                        \
+            __VA_ARGS__                                                                                                \
+        }                                                                                                              \
+    } while (0)
+
+// The step into arrays (the parity probes unc_fm_step / emu_fm_step): (ns[c], ne[c]) for all four bases; returns the
+// mask of the wanted bases whose range is non-empty
+UNC_DEV u32 unc_occ2_neighbors(const DevIndex &ix, u32 st, u32 en, u32 want, u32 ns[4], u32 ne[4], u32 *blocks) {
+    u32 valid = 0;
+    UNC_OCC2_STEP(ix, st, en, want, *blocks, ns[b] = nsb; ne[b] = neb; if (vb) valid |= 1u << b;);
+    return valid;
+}
+
 // ---- sort keys -----------------------------------------------------------------------------------------
 // key = (fm_start, fm_end, seed_prob bits, seedable | move_count << 1 | k-mer's position in a merged group << 6 | record index << 14)
 // order: fm_start, fm_end, seed_prob, record index (= emission order) -- reference src/mapper.cpp:866-871 plus
@@ -509,29 +551,9 @@ UNC_DEV void unc_k2_workers_v2(const DevIndex &ix, const DevParams &p, const Dev
                 }
                 if (cmask) stage_r[(u32) lane * 5u] = make_uint2(st, en);
                 if (want) {
-                    // BwaIndex::get_neighbor (reference src/bwa_index.hpp:158-162) over bwt_2occ (submods/bwa/bwt.c:132-163)
-                    // for all four bases: ns = L2[c] + Occ(start-1, c) + 1, ne = L2[c] + Occ(end, c)
-                    const u32 k0 = st - 1u, l0 = en;
-                    const u32 kk = k0 - (k0 >= ix.primary), ll = l0 - (l0 >= ix.primary);
-                    const bool l_is_end = (l0 == ix.seq_len);
-                    const uint4 *bk = ix.occ2 + ((size_t) (kk >> 6) << 1);
-                    const uint4 kc = d_ldg(bk), ks = d_ldg(bk + 1);
-                    uint4 lc = kc, ls = ks;
-                    if (!l_is_end && (ll >> 6) != (kk >> 6)) {
-                        const uint4 *bl = ix.occ2 + ((size_t) (ll >> 6) << 1);
-                        lc = d_ldg(bl); ls = d_ldg(bl + 1);
-                    }
-                    pend_blocks += 1u + ((!l_is_end && (ll >> 7) != (kk >> 7)) ? 1u : 0u);   // in the reference's 128-row blocks
-                    u32 ok[4], ol[4];
-                    unc_occ2_all(kc, ks, kk & 63u, ok);
-                    unc_occ2_all(lc, ls, ll & 63u, ol);
-                    if (l_is_end) { ol[0] = ix.L2[1] - ix.L2[0]; ol[1] = ix.L2[2] - ix.L2[1]; ol[2] = ix.L2[3] - ix.L2[2]; ol[3] = ix.L2[4] - ix.L2[3]; }
                     // a valid child's range goes to the parent's fixed staging slot lane*5 + 1 + base at once
-#pragma unroll
-                    for (u32 b = 0; b < 4; b++) {
-                        const u32 nsb = ix.L2[b] + ok[b] + 1u, neb = ix.L2[b] + ol[b];
-                        if (((want >> b) & 1u) && nsb <= neb) { cmask |= 2u << b; stage_r[(u32) lane * 5u + 1u + b] = make_uint2(nsb, neb); }
-                    }
+                    UNC_OCC2_STEP(ix, st, en, want, pend_blocks,
+                                  if (vb) { cmask |= 2u << b; stage_r[(u32) lane * 5u + 1u + b] = make_uint2(nsb, neb); });
                 }
                 const u32 cc = (u32) d_popc(cmask);
                 u32 total;

@@ -58,6 +58,16 @@ class Index:
                                         os_.ctypes.data, oe.ctypes.data))
         return os_, oe
 
+    def fm_step(self, start, end, want):
+        """The mapper's backward step per entry: (ns, ne) of shape (n, 4) for all four bases, and the valid masks."""
+        start = np.ascontiguousarray(start, np.uint64)
+        end = np.ascontiguousarray(end, np.uint64)
+        want = np.ascontiguousarray(want, np.uint8)
+        ns, ne, valid = np.zeros((len(start), 4), np.uint64), np.zeros((len(start), 4), np.uint64), np.zeros_like(want)
+        N.check(self.L.unc_fm_step(self.h, len(start), start.ctypes.data, end.ctypes.data, want.ctypes.data,
+                                   ns.ctypes.data, ne.ctypes.data, valid.ctypes.data))
+        return ns, ne, valid
+
     def sa(self, rows):
         rows = np.ascontiguousarray(rows, np.uint64)
         out = np.zeros_like(rows)
