@@ -347,6 +347,25 @@ int unc_self_align(const char *bwa_prefix, uint32_t sample_dist, uint64_t *n_pat
                    uint64_t **values);
 void unc_free(void *p);
 
+/* ---- repeat length of every reference position (`find-repeats`) ------------------------------------------------
+ *   unc_repeats_create    BwaIndex fmi(bwa_prefix); fmi.load_pacseq()           src/find_repeats.cpp:37,61-62
+ *   unc_repeats_lengths   the walk from every position of a window               src/find_repeats.cpp:61-85,
+ *                                                                                src/self_align_ref.cpp:64-84
+ *   unc_repeats_destroy
+ * The repeat length L(p) of .pac position p is the number of get_neighbor steps of self_align's walk from p
+ * (src/bwa_index.hpp:158-174): r = get_base_range(comp(b(p))); then r = get_neighbor(r, comp(b(j))) for j = p + 1, ...
+ * while j is before the end of p's contig and r.length() > 1, with b(q) the .pac base at q (src/bwa_index.hpp:257-259).
+ * find_repeats.cpp prints L as j - i; it extends with uncomplemented bases, which search the reversed strand, so its
+ * own walk is not reproduced.  create loads <prefix>.bwt / .sa / .ann / .pac (no .uncl); contigs are back to back in
+ * .ann order.  unc_repeats_lengths writes out[i] = L(pac_st + i) for i < n; a walk may run past the window to the end
+ * of its contig.  UNC_E_ARG for a window past the end of the reference, UNC_E_TOO_LARGE for 2^32 - 256 FM rows or
+ * more.  unc_repeats_last_kernel_ms: CUDA-event time of the last window's kernel. */
+typedef struct unc_repeats unc_repeats;
+int unc_repeats_create(const char *bwa_prefix, unc_repeats **out);
+int unc_repeats_lengths(unc_repeats *r, uint64_t pac_st, uint32_t n, uint32_t *out);
+int unc_repeats_last_kernel_ms(const unc_repeats *r, float *ms);
+void unc_repeats_destroy(unc_repeats *r);
+
 /* ---- DTW of event means against reference k-mers (analysis; SURVEY section 8(f) rank 4) ----------------------
  *   unc_dtw_batch       DTWr94p(means, kmers, prms) / DTWr94d(...) + get_path() / score()
  *                                                      src/dtw.hpp:31-183 (DTW<float, u16, Func>), :188-232 (the two

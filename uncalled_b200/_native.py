@@ -99,7 +99,8 @@ EXPORTS = ["unc_strerror", "unc_last_error", "unc_device_count", "unc_init", "un
            "unc_dtw_aligner_set_budget", "unc_dtw_align_batch", "unc_dtw_align_path", "unc_dtw_align_last_times",
            "unc_debug_held", "unc_dtw_batch_banded", "unc_dtw_aligner_set_band", "unc_event_params_default", "unc_events_create",
            "unc_events_free", "unc_events_run", "unc_events_fetch", "unc_events_annotate", "unc_match_probs_batch",
-           "unc_events_last_times"]
+           "unc_events_last_times", "unc_repeats_create", "unc_repeats_lengths", "unc_repeats_last_kernel_ms",
+           "unc_repeats_destroy"]
 
 
 def build(force=False, verbose=False):
@@ -108,7 +109,7 @@ def build(force=False, verbose=False):
     srcs = [os.path.join(src_dir, f) for f in ("unc_abi.cu", "unc_index_build.cpp", "unc_fast5.cpp")]
     deps = srcs + [os.path.join(src_dir, f) for f in
                    ("unc_device.cuh", "unc_k2v2.cuh", "unc_dtw.cuh", "unc_dtw_band.cuh", "unc_dtw_plan.hpp", "unc_dtw_host.inl", "unc_dtw_align.cuh", "unc_dtw_align_host.inl", "unc_k1.cuh", "unc_stream.cuh", "unc_stream_host.inl", "unc_stream_logic.hpp", "unc_replay.cuh", "unc_replay_host.inl", "unc_events.cuh", "unc_events_host.inl", "unc_ordered_logic.hpp", "unc_pdqsort.cuh", "unc_warp.cuh",
-                    "unc_selfalign.cuh", "unc_selfalign_host.hpp", "unc_selfalign_host.inl",
+                    "unc_selfalign.cuh", "unc_selfalign_host.hpp", "unc_selfalign_host.inl", "unc_repeats_host.inl",
                     "unc_mask.cuh", "unc_mask_host.hpp", "unc_mask_host.inl",
                     "unc_mask_ext.cuh", "unc_mask_ext_host.hpp", "unc_mask_ext_host.inl",
                     "unc_fmb.cuh", "unc_fmb_run.hpp", "unc_fmb_host.inl", "unc_index_host.hpp",
@@ -240,6 +241,11 @@ def lib():
     L.unc_events_annotate.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]
     L.unc_match_probs_batch.argtypes = [vp, vp, u64, vp]
     L.unc_events_last_times.argtypes = [vp, C.POINTER(C.c_float)]
+    L.unc_repeats_create.argtypes = [C.c_char_p, C.POINTER(vp)]
+    L.unc_repeats_lengths.argtypes = [vp, u64, u32, vp]
+    L.unc_repeats_last_kernel_ms.argtypes = [vp, C.POINTER(C.c_float)]
+    L.unc_repeats_destroy.argtypes = [vp]
+    L.unc_repeats_destroy.restype = None
     _lib = L
     return L
 

@@ -153,6 +153,17 @@ def get_parser(conf):
     p.add_argument("--batch-reads", type=int, default=256, help="Reads per GPU batch")
     p.add_argument("--device", type=int, default=0, help="CUDA device")
 
+    p = sp.add_parser("find-repeats", help="Report how long the sequence at each reference position stays repeated in the "
+                      "reference and its reverse complement (src/find_repeats.cpp)", formatter_class=fmt,
+                      description="One line per position whose repeat length L is at least min_k: L, contig, p, p + L and "
+                      "the contig's bases [p, p + L) (N inside .amb holes).  L is the number of FM-index steps after "
+                      "which the bases from p are unique or the contig ends.  Positions inside .amb holes are not reported.")
+    p.add_argument("bwa_prefix", type=str, help="BWA prefix of the reference (.bwt, .sa, .pac, .ann and .amb are read)")
+    p.add_argument("min_k", type=int, help="report positions with a repeat length of at least this (0: every position)")
+    p.add_argument("--bed", action="store_true", help="write the merged intervals [p, p + L) of the reported positions as "
+                   "BED instead")
+    p.add_argument("--device", type=int, default=0, help="CUDA device")
+
     p = sp.add_parser("pafstats",help="Computes speed and accuracy of UNCALLED mappings.", formatter_class=fmt)
     p.add_argument("infile", type=str, help="PAF file output by UNCALLED")          # uncalled/pafstats.py:165-169
     p.add_argument("-n", "--max-reads", required=False, type=int, default=None, help="Will only look at first n reads if specified")
@@ -419,6 +430,26 @@ def events_cmd(args, out=None):
             out.flush()
 
 
+def find_repeats_cmd(args, out=None):
+    """`find-repeats`: the reported positions' lines, or their BED with --bed, on `out` (stdout).  A negative min_k or a
+    missing or inconsistent index ends the command with status 1 before the GPU is touched."""
+    from .repeats import IndexFileError, RepeatFinder, write_bed, write_lines
+    out = out or sys.stdout
+    if args.min_k < 0:
+        sys.stderr.write("Error: min_k must be 0 or more\n")
+        sys.exit(1)
+    try:
+        finder = RepeatFinder(args.bwa_prefix, device=args.device)
+    except IndexFileError as e:
+        sys.stderr.write("Error: %s\n" % e)
+        sys.exit(1)
+    try:
+        (write_bed if args.bed else write_lines)(finder, args.min_k, out)
+    finally:
+        finder.close()
+    out.flush()
+
+
 def _g9(a):
     """%.9g of every value of a float32 array (reads back to the same float32), as a list of strings"""
     return ["%.9g" % x for x in np.asarray(a, np.float64).tolist()]
@@ -479,6 +510,8 @@ def main(argv=None):
         dtw_cmd(args)
     elif args.subcmd == "events":
         events_cmd(args)
+    elif args.subcmd == "find-repeats":
+        find_repeats_cmd(args)
     elif args.subcmd == "pafstats":
         from . import pafstats
         pafstats.run(args.infile, args.ref_paf, args.max_reads)

@@ -973,6 +973,7 @@ int unc_debug_held(uint64_t *device_bytes, uint64_t *pinned_bytes, uint32_t *han
 #include "unc_stream_host.inl"
 #include "unc_replay_host.inl"
 #include "unc_selfalign_host.inl"
+#include "unc_repeats_host.inl"
 #include "unc_dtw_host.inl"
 #include "unc_dtw_align_host.inl"
 #include "unc_mask_host.inl"

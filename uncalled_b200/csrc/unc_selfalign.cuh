@@ -9,6 +9,9 @@
 // parks its first UNC_SA_STAGE lengths in a transposed staging array (value j of path i at j*n + i, so a
 // warp's stores coalesce); pass 2, after the host's prefix sum of the counts, copies the parked values to
 // their CSR places and re-walks only paths longer than the stage (repeats).
+//
+// `find-repeats` (reference src/find_repeats.cpp:61-85) runs the same walk from EVERY position and keeps only its
+// number of steps (unc_repeat_length, mode UNC_SA_STEPS): no per-position arrays, one u32 out per position.
 #pragma once
 #include "unc_device.cuh"
 
@@ -24,6 +27,21 @@ struct DevSelfAlign {
     u64 *values;            // out (pass 2)
 };
 
+// what unc_selfalign_walk does with the range lengths
+#define UNC_SA_PARK 0       // the first UNC_SA_STAGE go to park[j * n]; returns the number of lengths (pass 1)
+#define UNC_SA_WRITE 1      // every length goes to out[j]; returns the number of lengths (pass 2)
+#define UNC_SA_STEPS 2      // none is stored; returns the number of get_neighbor steps (find-repeats)
+
+// find-repeats over the .pac window [pac_st, pac_st + n): out[i] = steps of the walk from pac_st + i, which ends at
+// the end of its contig, the first of ends[0 .. n_contigs) above it (contigs back to back in .ann order)
+struct DevRepeats {
+    const u8 *pac;
+    const u32 *ends;
+    u32 n_contigs;
+    u32 pac_st, n;
+    u32 *out;
+};
+
 // complement of reference base p: BASE_COMP_B[get_base(p)] (src/bwa_index.hpp:257-259, src/bp.hpp)
 UNC_DEV u32 unc_pac_comp(const u8 *pac, u32 p) {
     return 3u - (((u32) d_ldg(pac + (p >> 2)) >> (((3u ^ p) & 3u) << 1)) & 3u);
@@ -37,12 +55,11 @@ UNC_DEV u32 unc_occ_row(const DevIndex &ix, u32 k, u32 c) {
     return unc_occ_at(ix.bwt + ((size_t) (kk >> 7) << 2), kk, c);
 }
 
-// Walks one path; returns the number of range lengths.  PARK: the first UNC_SA_STAGE lengths go to
-// park[j * n] (pass 1); otherwise every length goes to out[j] (pass 2).
+// Walks one path; MODE (UNC_SA_*) says what is kept and returned.
 // The first range is get_base_range(b) = [L2[b], L2[b+1]] -- its start is NOT L2[b]+1
 // (src/bwa_index.hpp:172-174), so row start-1 can be (u64)-1.  Lengths are u32 on the device
 // (the index image is limited to < 2^32 rows) with the same wrap-around to 0 for an empty range.
-template <bool PARK>
+template <int MODE>
 UNC_DEV u32 unc_selfalign_walk(const DevIndex &ix, const u8 *pac, u32 pos, u32 lim, u32 *park, u32 n_paths, u64 *out) {
     u32 b = unc_pac_comp(pac, pos);
     u32 rs = unc_L2(ix, b), re = unc_L2(ix, b + 1);
@@ -51,22 +68,21 @@ UNC_DEV u32 unc_selfalign_walk(const DevIndex &ix, const u8 *pac, u32 pos, u32 l
         const u32 len = re - rs + 1u;
         const bool go = j < lim && len > 1u;
         if (go || len > 0u) {                                        // empty only after an N-derived base
-            if (PARK) { if (n < UNC_SA_STAGE) park[(size_t) n * n_paths] = len; }
-            else out[n] = (u64) len;
+            if (MODE == UNC_SA_PARK) { if (n < UNC_SA_STAGE) park[(size_t) n * n_paths] = len; }
+            else if (MODE == UNC_SA_WRITE) out[n] = (u64) len;
             n++;
         }
-        if (!go) break;
+        if (!go) return MODE == UNC_SA_STEPS ? j - pos - 1u : n;
         b = unc_pac_comp(pac, j);
         const u32 base = unc_L2(ix, b);
         const u32 ns = base + unc_occ_row(ix, rs - 1u, b) + 1u;      // get_neighbor (src/bwa_index.hpp:158-162)
         const u32 ne = base + unc_occ_row(ix, re, b);
         rs = ns; re = ne;
     }
-    return n;
 }
 
 UNC_DEV void unc_selfalign_count(const DevIndex &ix, const DevSelfAlign &A, u32 i) {
-    A.count[i] = unc_selfalign_walk<true>(ix, A.pac, A.pos[i], A.lim[i], A.stage + i, A.n, nullptr);
+    A.count[i] = unc_selfalign_walk<UNC_SA_PARK>(ix, A.pac, A.pos[i], A.lim[i], A.stage + i, A.n, nullptr);
 }
 
 UNC_DEV void unc_selfalign_write(const DevIndex &ix, const DevSelfAlign &A, u32 i) {
@@ -75,6 +91,16 @@ UNC_DEV void unc_selfalign_write(const DevIndex &ix, const DevSelfAlign &A, u32 
     if (cnt <= UNC_SA_STAGE) {
         for (u32 j = 0; j < cnt; j++) out[j] = (u64) A.stage[(size_t) j * A.n + i];
     } else {
-        unc_selfalign_walk<false>(ix, A.pac, A.pos[i], A.lim[i], nullptr, 0, out);
+        unc_selfalign_walk<UNC_SA_WRITE>(ix, A.pac, A.pos[i], A.lim[i], nullptr, 0, out);
     }
+}
+
+UNC_DEV void unc_repeat_length(const DevIndex &ix, const DevRepeats &R, u32 i) {
+    const u32 p = R.pac_st + i;
+    u32 lo = 0, hi = R.n_contigs - 1u;                               // the first contig end above p
+    while (lo < hi) {
+        const u32 m = (lo + hi) >> 1;
+        if (d_ldg(R.ends + m) > p) hi = m; else lo = m + 1u;
+    }
+    R.out[i] = unc_selfalign_walk<UNC_SA_STEPS>(ix, R.pac, p, d_ldg(R.ends + lo), nullptr, 0, nullptr);
 }

@@ -51,3 +51,12 @@ static inline void unc_selfalign_sample(const std::vector<uint32_t> &seq_lens, u
         st += len;
     }
 }
+
+// find-repeats: the .pac end (exclusive) of every sequence, sequences laid out back to back as above.  Zero-length
+// sequences give repeated ends, which the device's search for the first end above a position skips.
+static inline std::vector<uint32_t> unc_repeats_ends(const std::vector<uint32_t> &seq_lens) {
+    std::vector<uint32_t> ends;
+    uint64_t st = 0;
+    for (uint32_t len : seq_lens) ends.push_back((uint32_t) (st += len));
+    return ends;
+}
