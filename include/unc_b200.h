@@ -366,6 +366,48 @@ int unc_repeats_lengths(unc_repeats *r, uint64_t pac_st, uint32_t n, uint32_t *o
 int unc_repeats_last_kernel_ms(const unc_repeats *r, float *ms);
 void unc_repeats_destroy(unc_repeats *r);
 
+/* ---- the reference's BwaIndex queries (src/bwa_index.hpp:103-333) ------------------------------------------------
+ *   unc_bwa_open          BwaIndex(prefix, pacseq): reads .bwt .sa .ann .amb (+ .pac when load_pac), never .uncl.
+ *                         Host only: the device image (the find-repeats image plus the sampled SA) is built by the
+ *                         first query that runs on the device, on `device`.  UNC_E_IO for a missing or
+ *                         inconsistent file, UNC_E_TOO_LARGE from 2^32 - 256 FM rows.
+ *   unc_bwa_load_pac      load_pacseq (a no-op when loaded)
+ *   unc_bwa_info          size() (seq_len = 2 l_pac), l_pac, the number of contigs and L2[0..4]
+ *   unc_bwa_seq           contig rid's name (valid while the handle lives), .pac offset and length (.ann order)
+ *   unc_bwa_kmer_ranges   the 1024 k-mer ranges of load_index (get_base_range quirk included)
+ *   unc_bwa_pos2rid       bns_pos2rid: the contig holding .pac position pos, -1 past l_pac
+ *   unc_bwa_coord_to_pacseq  offset + coord, INT_MAX for an unknown name (as the reference)
+ *   unc_bwa_get_base      base i of the .pac (needs the .pac; UNC_E_ARG for i >= l_pac)
+ * Device queries, n items in, n results out:
+ *   unc_bwa_neighbor      get_neighbor over bwt_2occ as bwa writes it, inverted ranges computed, not rejected.
+ *                         UNC_E_ARG for start > size() + 1, end > size() or base > 3 (reads past the index)
+ *   unc_bwa_sa            bwt_sa; row 0 gives (u64)-1; UNC_E_ARG for a row above size()
+ *   unc_bwa_range_to_fms  range_to_fms(name, start, end): out_first[end - start] = the reference's first list (rows of
+ *                         positions pac_min .. pac_max, reverse walk), out_second[end - start] = its second (pac_max
+ *                         down to pac_min, forward walk).  UNC_E_ARG, before the device is touched, for an unknown
+ *                         name, end <= start, pac_max >= l_pac or no .pac; UNC_E_IO if a segment's anchor row is not
+ *                         found (an index whose .pac and .bwt disagree).
+ *   unc_bwa_get_kmers     get_kmers(pac_st, pac_en) = seq_to_kmers: out[max(0, pac_en - pac_st - 4)] k-mers of
+ *                         bases [pac_st, pac_en).  UNC_E_ARG for pac_en > l_pac or no .pac.
+ *   unc_bwa_last_kernel_ms  CUDA-event time of the last device query's kernels */
+typedef struct unc_bwa unc_bwa;
+int unc_bwa_open(const char *bwa_prefix, int load_pac, int device, unc_bwa **out);
+void unc_bwa_free(unc_bwa *h);
+int unc_bwa_load_pac(unc_bwa *h);
+int unc_bwa_info(const unc_bwa *h, uint64_t *seq_len, uint64_t *l_pac, int32_t *n_seqs, int32_t *pac_loaded, uint64_t L2[5]);
+int unc_bwa_seq(const unc_bwa *h, int32_t rid, const char **name, uint64_t *offset, uint64_t *len);
+int unc_bwa_kmer_ranges(unc_bwa *h, uint64_t *starts, uint64_t *ends);
+int32_t unc_bwa_pos2rid(const unc_bwa *h, uint64_t pos);
+int unc_bwa_coord_to_pacseq(const unc_bwa *h, const char *name, uint64_t coord, uint64_t *out);
+int unc_bwa_get_base(const unc_bwa *h, uint64_t i, uint8_t *out);
+int unc_bwa_neighbor(unc_bwa *h, uint64_t n, const uint64_t *starts, const uint64_t *ends, const uint8_t *bases,
+                     uint64_t *out_starts, uint64_t *out_ends);
+int unc_bwa_sa(unc_bwa *h, uint64_t n, const uint64_t *rows, uint64_t *out);
+int unc_bwa_range_to_fms(unc_bwa *h, const char *name, uint64_t start, uint64_t end, uint64_t *out_first,
+                         uint64_t *out_second);
+int unc_bwa_get_kmers(unc_bwa *h, uint64_t pac_st, uint64_t pac_en, uint16_t *out);
+int unc_bwa_last_kernel_ms(const unc_bwa *h, float *ms);
+
 /* ---- DTW of event means against reference k-mers (analysis; SURVEY section 8(f) rank 4) ----------------------
  *   unc_dtw_batch       DTWr94p(means, kmers, prms) / DTWr94d(...) + get_path() / score()
  *                                                      src/dtw.hpp:31-183 (DTW<float, u16, Func>), :188-232 (the two

@@ -100,7 +100,9 @@ EXPORTS = ["unc_strerror", "unc_last_error", "unc_device_count", "unc_init", "un
            "unc_debug_held", "unc_dtw_batch_banded", "unc_dtw_aligner_set_band", "unc_event_params_default", "unc_events_create",
            "unc_events_free", "unc_events_run", "unc_events_fetch", "unc_events_annotate", "unc_match_probs_batch",
            "unc_events_last_times", "unc_repeats_create", "unc_repeats_lengths", "unc_repeats_last_kernel_ms",
-           "unc_repeats_destroy"]
+           "unc_repeats_destroy", "unc_bwa_open", "unc_bwa_free", "unc_bwa_load_pac", "unc_bwa_info", "unc_bwa_seq",
+           "unc_bwa_kmer_ranges", "unc_bwa_pos2rid", "unc_bwa_coord_to_pacseq", "unc_bwa_get_base", "unc_bwa_neighbor",
+           "unc_bwa_sa", "unc_bwa_range_to_fms", "unc_bwa_get_kmers", "unc_bwa_last_kernel_ms"]
 
 
 def build(force=False, verbose=False):
@@ -109,7 +111,7 @@ def build(force=False, verbose=False):
     srcs = [os.path.join(src_dir, f) for f in ("unc_abi.cu", "unc_index_build.cpp", "unc_fast5.cpp")]
     deps = srcs + [os.path.join(src_dir, f) for f in
                    ("unc_device.cuh", "unc_k2v2.cuh", "unc_dtw.cuh", "unc_dtw_band.cuh", "unc_dtw_plan.hpp", "unc_dtw_host.inl", "unc_dtw_align.cuh", "unc_dtw_align_host.inl", "unc_k1.cuh", "unc_stream.cuh", "unc_stream_host.inl", "unc_stream_logic.hpp", "unc_replay.cuh", "unc_replay_host.inl", "unc_events.cuh", "unc_events_host.inl", "unc_ordered_logic.hpp", "unc_pdqsort.cuh", "unc_warp.cuh",
-                    "unc_selfalign.cuh", "unc_selfalign_host.hpp", "unc_selfalign_host.inl", "unc_repeats_host.inl",
+                    "unc_selfalign.cuh", "unc_selfalign_host.hpp", "unc_selfalign_host.inl", "unc_repeats_host.inl", "unc_bwa.cuh", "unc_bwa_host.inl",
                     "unc_mask.cuh", "unc_mask_host.hpp", "unc_mask_host.inl",
                     "unc_mask_ext.cuh", "unc_mask_ext_host.hpp", "unc_mask_ext_host.inl",
                     "unc_fmb.cuh", "unc_fmb_run.hpp", "unc_fmb_host.inl", "unc_index_host.hpp",
@@ -246,6 +248,22 @@ def lib():
     L.unc_repeats_last_kernel_ms.argtypes = [vp, C.POINTER(C.c_float)]
     L.unc_repeats_destroy.argtypes = [vp]
     L.unc_repeats_destroy.restype = None
+    L.unc_bwa_open.argtypes = [C.c_char_p, C.c_int, C.c_int, C.POINTER(vp)]
+    L.unc_bwa_free.argtypes = [vp]
+    L.unc_bwa_free.restype = None
+    L.unc_bwa_load_pac.argtypes = [vp]
+    L.unc_bwa_info.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(C.c_int32), C.POINTER(C.c_int32), vp]
+    L.unc_bwa_seq.argtypes = [vp, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(u64), C.POINTER(u64)]
+    L.unc_bwa_kmer_ranges.argtypes = [vp, vp, vp]
+    L.unc_bwa_pos2rid.argtypes = [vp, u64]
+    L.unc_bwa_pos2rid.restype = C.c_int32
+    L.unc_bwa_coord_to_pacseq.argtypes = [vp, C.c_char_p, u64, C.POINTER(u64)]
+    L.unc_bwa_get_base.argtypes = [vp, u64, C.POINTER(C.c_uint8)]
+    L.unc_bwa_neighbor.argtypes = [vp, u64, vp, vp, vp, vp, vp]
+    L.unc_bwa_sa.argtypes = [vp, u64, vp, vp]
+    L.unc_bwa_range_to_fms.argtypes = [vp, C.c_char_p, u64, u64, vp, vp]
+    L.unc_bwa_get_kmers.argtypes = [vp, u64, u64, vp]
+    L.unc_bwa_last_kernel_ms.argtypes = [vp, C.POINTER(C.c_float)]
     _lib = L
     return L
 

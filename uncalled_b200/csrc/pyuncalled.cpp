@@ -13,7 +13,10 @@
 #include <pybind11/pybind11.h>
 #include <pybind11/stl.h>
 
+#include <algorithm>
 #include <chrono>
+#include <climits>
+#include <tuple>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -368,11 +371,196 @@ class RealtimePool {
 };
 
 // ------------------------------------------------------------------ index side
+// Range (reference src/range.hpp:34-68, src/range.cpp)
+struct Range {
+    u64 start_ = 1, end_ = 0;
+    Range() = default;
+    Range(u64 s, u64 e) : start_(s), end_(e) {}
+    bool is_valid() const { return start_ <= end_; }
+    u64 length() const { return end_ - start_ + 1; }
+    bool intersects(const Range &q) const {
+        return is_valid() && q.is_valid() && !(start_ > q.end_ || end_ < q.start_) && !(q.start_ > end_ || q.end_ < start_);
+    }
+    Range intersect(const Range &r) const { return intersects(r) ? Range(std::max(start_, r.start_), std::min(end_, r.end_)) : Range(); }
+    Range merge(const Range &r) const { return intersects(r) ? Range(std::min(start_, r.start_), std::max(end_, r.end_)) : Range(); }
+    float get_recp_overlap(const Range &r) const {
+        return intersects(r) ? float(intersect(r).length()) / float(merge(r).length()) : 0.f;
+    }
+    Range split_range(const Range &r) {
+        Range left;
+        if (start_ < r.start_) { left = *this; left.end_ = r.start_ - 1; }
+        if (start_ <= r.end_) {
+            if (end_ > r.end_) start_ = r.end_ + 1;
+            else { start_ = 1; end_ = 0; }
+        }
+        return left;
+    }
+    bool same_range(const Range &q) const { return start_ == q.start_ && end_ == q.end_; }
+    bool operator<(const Range &q) const { return start_ < q.start_ || (start_ == q.start_ && end_ < q.end_); }
+    bool operator==(const Range &q) const { return same_range(q); }
+};
+
+// k-mer helpers of src/bp.hpp for k = 5
+static const u8 KLEN = 5;
+static u16 kmer_count() { return 1024; }
+static u16 str_to_kmer(const std::string &kmer, u64 offset) {
+    auto b = [](char c) -> u16 {
+        switch (c) { case 'A': case 'a': return 0; case 'C': case 'c': return 1; case 'G': case 'g': return 2;
+                     case 'T': case 't': return 3; default: return 4; }
+    };
+    if (offset + KLEN > kmer.size()) throw std::out_of_range("k-mer string too short");
+    u16 index = b(kmer[offset]);
+    for (u8 i = 1; i < KLEN; i++) index = (u16) ((index << 2) | b(kmer[offset + i]));
+    return index;
+}
+static u16 kmer_comp(u16 kmer) { return kmer ^ 0x3FF; }
+static u16 kmer_revcomp(u16 kmer) {          // complement, then reverse the order of the 2-bit bases
+    u16 x = (kmer ^ 0x3FF) & 0x3FF, r = 0;
+    for (u8 i = 0; i < KLEN; i++) { r = (u16) ((r << 2) | (x & 3)); x >>= 2; }
+    return r;
+}
+static u8 kmer_head(u16 kmer) { return (u8) ((kmer >> (2 * KLEN - 2)) & 3); }
+static u16 kmer_neighbor(u16 kmer, u8 i) { return (u16) (((kmer << 2) & 0x3FF) | i); }
+static u8 kmer_base(u16 kmer, u8 i) {
+    if (i >= KLEN) throw std::out_of_range("base index outside the k-mer");
+    return (u8) ((kmer >> (2 * (KLEN - i - 1))) & 3);
+}
+static std::string kmer_to_str(u16 kmer) {
+    std::string s(KLEN, 'N');
+    for (u8 i = 0; i < KLEN; i++) s[i] = "ACGT"[kmer_base(kmer, i)];
+    return s;
+}
+
+// BwaIndex<5> (reference src/bwa_index.hpp:88-377) over unc_bwa_*: FM-index queries on the GPU, the rest on the host
 struct BwaIndex {
+    unc_bwa *h_ = nullptr;
+    std::vector<Range> kr_;
+    BwaIndex() = default;
+    BwaIndex(const std::string &prefix, bool pacseq) {
+        if (!prefix.empty()) load_index(prefix);
+        if (pacseq) load_pacseq();
+    }
+    ~BwaIndex() { destroy(); }
+    BwaIndex(const BwaIndex &) = delete;
+    BwaIndex &operator=(const BwaIndex &) = delete;
+
     static void create(const std::string &fasta, const std::string &prefix) {        // BwaIndex::create, src/bwa_index.hpp:92-101
         // the device builder where a CUDA device is visible; both write the same files
         if (unc_device_count() > 0) check(unc_index_build_device(fasta.c_str(), prefix.c_str()), "unc_index_build_device");
         else check(unc_index_build(fasta.c_str(), prefix.c_str()), "unc_index_build");
+    }
+    void load_index(const std::string &prefix) {
+        destroy();
+        check(unc_bwa_open(prefix.c_str(), 0, 0, &h_), "unc_bwa_open");
+    }
+    bool is_loaded() const { return h_ != nullptr; }
+    unc_bwa *hd() const {
+        if (!h_) throw std::runtime_error("no index loaded");
+        return h_;
+    }
+    void load_pacseq() { check(unc_bwa_load_pac(hd()), "unc_bwa_load_pac"); }
+    bool pacseq_loaded() const {
+        int32_t pl = 0;
+        if (h_) check(unc_bwa_info(h_, nullptr, nullptr, nullptr, &pl, nullptr), "unc_bwa_info");
+        return pl != 0;
+    }
+    void destroy() {
+        if (h_) unc_bwa_free(h_);
+        h_ = nullptr;
+        kr_.clear();
+    }
+    Range get_neighbor(Range r, u8 base) const {
+        u64 s, e;
+        check(unc_bwa_neighbor(hd(), 1, &r.start_, &r.end_, &base, &s, &e), "unc_bwa_neighbor");
+        return Range(s, e);
+    }
+    const std::vector<Range> &kmer_ranges() {
+        if (kr_.empty()) {
+            std::vector<u64> st(1024), en(1024);
+            check(unc_bwa_kmer_ranges(hd(), st.data(), en.data()), "unc_bwa_kmer_ranges");
+            for (int k = 0; k < 1024; k++) kr_.emplace_back(st[k], en[k]);
+        }
+        return kr_;
+    }
+    Range get_kmer_range(u16 kmer) { return kmer_ranges().at(kmer); }
+    u64 get_kmer_count(u16 kmer) { return get_kmer_range(kmer).length(); }
+    u64 L2(int b) const {
+        u64 l2[5];
+        check(unc_bwa_info(hd(), nullptr, nullptr, nullptr, nullptr, l2), "unc_bwa_info");
+        return l2[b];
+    }
+    Range get_base_range(u8 base) const {
+        if (base > 3) throw std::out_of_range("base above 3");
+        return Range(L2(base), L2(base + 1));
+    }
+    u64 sa(u64 i) const {
+        u64 v;
+        check(unc_bwa_sa(hd(), 1, &i, &v), "unc_bwa_sa");
+        return v;
+    }
+    u64 size() const {
+        u64 n;
+        check(unc_bwa_info(hd(), &n, nullptr, nullptr, nullptr, nullptr), "unc_bwa_info");
+        return n;
+    }
+    void seq(int rid, const char **name, u64 *off, u64 *len) const { check(unc_bwa_seq(hd(), rid, name, off, len), "unc_bwa_seq"); }
+    int get_rid(u64 sa_loc) const { return unc_bwa_pos2rid(hd(), sa_loc); }
+    std::pair<int, u32> get_ref_coord(u64 sa_loc) const {
+        const int rid = get_rid(sa_loc);
+        u64 off;
+        seq(rid, nullptr, &off, nullptr);
+        return {rid, (u32) (sa_loc - off)};
+    }
+    std::string get_ref_name(int rid) const { const char *nm; seq(rid, &nm, nullptr, nullptr); return nm; }
+    u64 get_ref_len(int rid) const { u64 len; seq(rid, nullptr, nullptr, &len); return len; }
+    u64 get_sa_loc(const std::string &name, u64 coord) const {
+        const u64 p = coord_to_pacseq(name, coord);
+        return p == (u64) INT_MAX && !has_seq(name) ? 0 : p;
+    }
+    bool has_seq(const std::string &name) const {
+        int32_t n = 0;
+        check(unc_bwa_info(hd(), nullptr, nullptr, &n, nullptr, nullptr), "unc_bwa_info");
+        for (int i = 0; i < n; i++) if (get_ref_name(i) == name) return true;
+        return false;
+    }
+    // translate_loc(sa_loc, &ref_name, &ref_loc) returns through its arguments in C++: here (ref_len, ref_name, ref_loc)
+    std::tuple<u64, std::string, u64> translate_loc(u64 sa_loc) const {
+        const int rid = get_rid(sa_loc);
+        if (rid < 0) return std::make_tuple((u64) 0, std::string(), (u64) 0);
+        const char *nm;
+        u64 off, len;
+        seq(rid, &nm, &off, &len);
+        return std::make_tuple(len, std::string(nm), sa_loc - off);
+    }
+    std::vector<std::pair<std::string, u64>> get_seqs() const {
+        int32_t n = 0;
+        check(unc_bwa_info(hd(), nullptr, nullptr, &n, nullptr, nullptr), "unc_bwa_info");
+        std::vector<std::pair<std::string, u64>> ret;
+        for (int i = 0; i < n; i++) ret.emplace_back(get_ref_name(i), get_ref_len(i));
+        return ret;
+    }
+    u64 coord_to_pacseq(const std::string &name, u64 coord) const {
+        u64 p;
+        check(unc_bwa_coord_to_pacseq(hd(), name.c_str(), coord, &p), "unc_bwa_coord_to_pacseq");
+        return p;
+    }
+    u8 get_base(u64 i) const {
+        u8 b;
+        check(unc_bwa_get_base(hd(), i, &b), "unc_bwa_get_base");
+        return b;
+    }
+    std::vector<u16> get_kmers(u64 st, u64 en) {
+        std::vector<u16> ret(en > st + 4 ? en - st - 4 : 0);
+        check(unc_bwa_get_kmers(hd(), st, en, ret.data()), "unc_bwa_get_kmers");
+        return ret;
+    }
+    std::vector<u16> get_kmers_named(std::string nm, u64 st, u64 en) { return get_kmers(coord_to_pacseq(nm, st), coord_to_pacseq(nm, en)); }
+    std::pair<std::vector<u64>, std::vector<u64>> range_to_fms(std::string ref_name, u64 start, u64 end) {
+        const u64 n = end > start ? end - start : 0;
+        std::vector<u64> first(n ? n : 1), second(n ? n : 1);
+        check(unc_bwa_range_to_fms(hd(), ref_name.c_str(), start, end, first.data(), second.data()), "unc_bwa_range_to_fms");
+        first.resize(n); second.resize(n);
+        return {first, second};
     }
 };
 static std::vector<std::vector<u64>> self_align(const std::string &prefix, u32 sample_dist) {   // src/self_align_ref.cpp:34-91
@@ -605,7 +793,50 @@ PYBIND11_MODULE(_uncalled, m) {
     py::enum_<RealtimePool::ActiveChs>(rp, "ActiveChs").value("FULL", RealtimePool::FULL).value("EVEN", RealtimePool::EVEN).value("ODD", RealtimePool::ODD).export_values();
 
     py::class_<ClientSim>(m, "ClientSim").def(py::init<Conf &>());
-    py::class_<BwaIndex>(m, "BwaIndex").def_static("create", &BwaIndex::create);
+    py::class_<Range>(m, "Range")
+        .def(py::init<>()).def(py::init<u64, u64>()).def(py::init<const Range &>())
+        .def_readwrite("start", &Range::start_).def_readwrite("end", &Range::end_)
+        .def("length", &Range::length).def("is_valid", &Range::is_valid).def("intersect", &Range::intersect)
+        .def("merge", &Range::merge).def("split_range", &Range::split_range).def("same_range", &Range::same_range)
+        .def("intersects", &Range::intersects).def("get_recp_overlap", &Range::get_recp_overlap)
+        .def("__lt__", &Range::operator<).def("__eq__", &Range::operator==)
+        .def("__repr__", [](const Range &r) { return "Range(" + std::to_string(r.start_) + ", " + std::to_string(r.end_) + ")"; });
+    // the method list of BwaIndex<KLEN>::pybind_defs (reference src/bwa_index.hpp:339-365)
+    py::class_<BwaIndex>(m, "BwaIndex")
+        .def(py::init<>())
+        .def(py::init<const std::string &, bool>())
+        .def_static("create", &BwaIndex::create)
+        .def("load_index", &BwaIndex::load_index)
+        .def("is_loaded", &BwaIndex::is_loaded)
+        .def("load_pacseq", &BwaIndex::load_pacseq)
+        .def("destroy", &BwaIndex::destroy)
+        .def("get_neighbor", &BwaIndex::get_neighbor)
+        .def("get_kmer_range", &BwaIndex::get_kmer_range)
+        .def("get_kmer_count", &BwaIndex::get_kmer_count)
+        .def("get_base_range", &BwaIndex::get_base_range)
+        .def("sa", &BwaIndex::sa)
+        .def("size", &BwaIndex::size)
+        .def("translate_loc", &BwaIndex::translate_loc)
+        .def("get_seqs", &BwaIndex::get_seqs)
+        .def("coord_to_pacseq", &BwaIndex::coord_to_pacseq)
+        .def("pacseq_loaded", &BwaIndex::pacseq_loaded)
+        .def("get_base", &BwaIndex::get_base)
+        .def("get_rid", &BwaIndex::get_rid)
+        .def("get_sa_loc", &BwaIndex::get_sa_loc)
+        .def("get_ref_coord", &BwaIndex::get_ref_coord)
+        .def("get_ref_name", &BwaIndex::get_ref_name)
+        .def("get_ref_len", &BwaIndex::get_ref_len)
+        .def("range_to_fms", &BwaIndex::range_to_fms)
+        .def("get_kmers", &BwaIndex::get_kmers)
+        .def("get_kmers", &BwaIndex::get_kmers_named);
+    m.def("kmer_count", &kmer_count);
+    m.def("str_to_kmer", &str_to_kmer, py::arg("kmer"), py::arg("offset") = 0);
+    m.def("kmer_comp", &kmer_comp);
+    m.def("kmer_revcomp", &kmer_revcomp);
+    m.def("kmer_head", &kmer_head);
+    m.def("kmer_base", &kmer_base);
+    m.def("kmer_to_str", &kmer_to_str);
+    m.def("kmer_neighbor", &kmer_neighbor);
     m.def("self_align", &self_align);
 
     py::class_<DTWr94<0>>(m, "DTWr94p").def(py::init<const std::vector<float> &, const std::vector<uint16_t> &, const DTWParams &>())

@@ -976,6 +976,7 @@ int unc_debug_held(uint64_t *device_bytes, uint64_t *pinned_bytes, uint32_t *han
 #include "unc_repeats_host.inl"
 #include "unc_dtw_host.inl"
 #include "unc_dtw_align_host.inl"
+#include "unc_bwa_host.inl"
 #include "unc_mask_host.inl"
 #include "unc_mask_ext_host.inl"
 #include "unc_fmb_host.inl"
